@@ -75,7 +75,7 @@ class JoinAgg(C.Structure):
 class StarLookup(C.Structure):
     _fields_ = [("dense", C.c_int32), ("pad_", C.c_int32), ("lookup", C.c_void_p), ("kmin", C.c_int64),
                 ("range", C.c_int64), ("table_keys", C.c_void_p), ("table_slots", C.c_void_p),
-                ("cap", C.c_int64)]
+                ("cap", C.c_int64), ("dir", C.c_void_p)]
 
 
 MAX_PEERS, PEER_MAX_ARRAYS = 16, 2 * MAX_AGGS + 1
@@ -94,7 +94,7 @@ class PeerMerge(C.Structure):
 
 assert C.sizeof(Col) == 24 and C.sizeof(Term) == 32 and C.sizeof(Scan) == 656
 assert C.sizeof(AggState) == 152 and C.sizeof(Instr) == 24 and C.sizeof(Prog) == 1544
-assert C.sizeof(JoinTable) == 152 and C.sizeof(StarLookup) == 56 and C.sizeof(PeerMerge) == 544
+assert C.sizeof(JoinTable) == 152 and C.sizeof(StarLookup) == 64 and C.sizeof(PeerMerge) == 544
 
 
 class B200SqlError(RuntimeError):
@@ -183,7 +183,9 @@ _SIGS = {
     "b2_sort_by": [C.POINTER(Col), C.c_int64, C.c_int32, C.c_int32, _P, _P, _P],
     "b2_dense_slots": [C.POINTER(Col), C.c_int64, C.c_int64, C.c_int32, _P, _P],
     "b2_star_build_dense": [C.POINTER(Col), _P, C.c_int64, _P, C.c_int64, C.c_int64, _P, _P, _P],
-    "b2_star_build_scan": [C.POINTER(Scan), C.c_int32, C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_int32, _P,
+    "b2_star_build_mark": [C.POINTER(Scan), C.c_int32, C.c_int64, C.c_int64, _P, _P, _P],
+    "b2_star_build_rank": [_P, C.c_int64, _P],
+    "b2_star_build_fill": [C.POINTER(Scan), C.c_int32, C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_int32, _P,
                            _P, _P],
     "b2_star_build_hash": [C.POINTER(Col), _P, C.c_int64, _P, _P, _P, C.c_int64, _P, _P],
     "b2_star_agg": [C.POINTER(Scan), C.c_int32, C.POINTER(StarLookup), C.POINTER(Agg), C.c_int32,
@@ -272,7 +274,9 @@ _lib.b2_sort_ws_bytes.argtypes = [C.c_int64]
 sort_ws_bytes = _lib.b2_sort_ws_bytes
 dense_slots = _wrap("b2_dense_slots")
 star_build_dense = _wrap("b2_star_build_dense")
-star_build_scan = _wrap("b2_star_build_scan")
+star_build_mark = _wrap("b2_star_build_mark")
+star_build_rank = _wrap("b2_star_build_rank")
+star_build_fill = _wrap("b2_star_build_fill")
 star_build_hash = _wrap("b2_star_build_hash")
 star_agg = _wrap("b2_star_agg")
 num_tiles = _lib.b2_num_tiles

@@ -191,11 +191,13 @@ b2_select_count_kernel(const __grid_constant__ b2_scan_t s, int64_t ntiles, int6
   }
 }
 
-// single-block exclusive scan of int64 counts in place; a[n] receives the total.
+// single-block exclusive scan in place: element i is read as io.get(i) and replaced by its exclusive
+// prefix through io.put(i, prefix); returns the total (in every thread).  Run by one block of
+// B2_SCAN_THREADS threads.
 #define B2_SCAN_THREADS 1024
 #define B2_SCAN_PER_THREAD 8
-__global__ void __launch_bounds__(B2_SCAN_THREADS)
-b2_exclusive_scan_kernel(int64_t* __restrict__ a, int64_t n) {
+template <class IO>
+__device__ __forceinline__ int64_t b2_block_exclusive_scan(const IO& io, int64_t n) {
   __shared__ int64_t warp_sums[32];
   __shared__ int64_t carry_sh;
   if (threadIdx.x == 0) carry_sh = 0;
@@ -208,7 +210,7 @@ b2_exclusive_scan_kernel(int64_t* __restrict__ a, int64_t n) {
     int64_t tsum = 0;
 #pragma unroll
     for (int k = 0; k < B2_SCAN_PER_THREAD; ++k) {
-      v[k] = (i0 + k < n) ? a[i0 + k] : 0;
+      v[k] = (i0 + k < n) ? io.get(i0 + k) : 0;
       tsum += v[k];
     }
     int64_t incl = tsum;
@@ -233,14 +235,27 @@ b2_exclusive_scan_kernel(int64_t* __restrict__ a, int64_t n) {
     int64_t excl = carry + (warp ? warp_sums[warp - 1] : 0) + (incl - tsum);
 #pragma unroll
     for (int k = 0; k < B2_SCAN_PER_THREAD; ++k) {
-      if (i0 + k < n) a[i0 + k] = excl;
+      if (i0 + k < n) io.put(i0 + k, excl);
       excl += v[k];
     }
     __syncthreads();
     if (threadIdx.x == B2_SCAN_THREADS - 1) carry_sh = carry + warp_sums[31];
     __syncthreads();
   }
-  if (threadIdx.x == 0) a[n] = carry_sh;
+  return carry_sh;
+}
+
+struct b2_scan_io_i64 {
+  int64_t* a;
+  __device__ int64_t get(int64_t i) const { return a[i]; }
+  __device__ void put(int64_t i, int64_t v) const { a[i] = v; }
+};
+
+// exclusive scan of int64 counts in place; a[n] receives the total.
+__global__ void __launch_bounds__(B2_SCAN_THREADS)
+b2_exclusive_scan_kernel(int64_t* __restrict__ a, int64_t n) {
+  const int64_t total = b2_block_exclusive_scan(b2_scan_io_i64{a}, n);
+  if (threadIdx.x == 0) a[n] = total;
 }
 
 struct b2_gather_arg {

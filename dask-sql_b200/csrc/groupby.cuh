@@ -266,13 +266,19 @@ b2_star_build_dense_kernel(const __grid_constant__ b2_col_t pk, const int32_t* _
   }
 }
 
-// Build side of the star pipeline in ONE pass when both the join key and the group key are dense:
-// predicate on the dimension partition -> group slot -> lookup[pk - kmin] = slot.  Nothing is
-// materialised (no selection vector, no filtered copy of the dimension table, no host sync).
+// Build side of the star pipeline straight from the UNFILTERED dimension partitions when both the join
+// key and the group key are dense: a ranked bitmap (include/b200sql.h, b2_starlookup_t.dir) instead of
+// an int32 per key, so that keys whose dimension row fails the predicate cost one bit of L2, not four
+// bytes.  Three steps over all partitions, in stream order, no host sync and nothing materialised:
+//   MARK  (every partition): predicate -> set the key's bit; a bit already set is a duplicate build key;
+//   rank  (once): exclusive scan of the words' popcounts into their rank fields;
+//   FILL  (every partition): predicate again -> slots[rank + set bits below the key's] = group slot.
+// The rank is global, so every partition's MARK must precede the scan.
+template <bool FILL>
 __global__ void __launch_bounds__(B2_BLOCK)
 b2_star_build_scan_kernel(const __grid_constant__ b2_scan_t s, int pk_col, int grp_col, int64_t pk_min,
-                          int64_t pk_range, int64_t grp_min, int32_t null_slot, int32_t* __restrict__ lookup,
-                          int32_t* __restrict__ flags) {
+                          int64_t pk_range, int64_t grp_min, int32_t null_slot, uint64_t* __restrict__ dir,
+                          int32_t* __restrict__ slots, int32_t* __restrict__ flags) {
   const int tile_off = (threadIdx.x >> 5) * (32 * B2_GB_R) + (threadIdx.x & 31);
   const b2_col_t& pc = s.cols[pk_col];
   const b2_col_t& gc = s.cols[grp_col];
@@ -281,22 +287,48 @@ b2_star_build_scan_kernel(const __grid_constant__ b2_scan_t s, int pk_col, int g
     const b2_gld ld{&s, base + tile_off};
     bool full;
     const uint32_t bits = b2_eval_terms<B2_GB_R>(s, ld, full);
-    int64_t pk[B2_GB_R], grp[B2_GB_R];
+    int64_t pk[B2_GB_R];
     ld.template load<B2_GB_R>(pk_col, bits, full, pk);
-    ld.template load<B2_GB_R>(grp_col, bits, full, grp);
     uint32_t live = bits;
     if (pc.valid) live &= b2_valid_bits<B2_GB_R>(pc.valid, ld.row0, bits);   // NULL keys never join
-    uint32_t gnull = 0;
-    if (gc.valid) gnull = bits & ~b2_valid_bits<B2_GB_R>(gc.valid, ld.row0, bits);
 #pragma unroll
     for (int j = 0; j < B2_GB_R; ++j) {
       const uint64_t d = (uint64_t)pk[j] - (uint64_t)pk_min;
-      if (((live >> j) & 1) && d < (uint64_t)pk_range) {
-        const int32_t slot = (gnull >> j) & 1 ? null_slot : (int32_t)(grp[j] - grp_min);
-        if (atomicExch(lookup + d, slot) != -1) flags[0] = 1;  // duplicate build key
+      if (!(((live >> j) & 1) && d < (uint64_t)pk_range)) live &= ~(1u << j);
+    }
+    if (!FILL) {
+#pragma unroll
+      for (int j = 0; j < B2_GB_R; ++j) {
+        if (!((live >> j) & 1)) continue;
+        const uint64_t d = (uint64_t)pk[j] - (uint64_t)pk_min;
+        const uint32_t b = 1u << (d & 31);
+        if (atomicOr(reinterpret_cast<uint32_t*>(dir + (d >> 5)), b) & b) flags[0] = 1;  // duplicate build key
+      }
+    } else {
+      int64_t grp[B2_GB_R];
+      ld.template load<B2_GB_R>(grp_col, live, false, grp);
+      uint32_t gnull = 0;
+      if (gc.valid) gnull = live & ~b2_valid_bits<B2_GB_R>(gc.valid, ld.row0, live);
+#pragma unroll
+      for (int j = 0; j < B2_GB_R; ++j) {
+        if (!((live >> j) & 1)) continue;
+        const uint64_t d = (uint64_t)pk[j] - (uint64_t)pk_min;
+        const uint64_t w = dir[d >> 5];
+        const uint32_t pos = (uint32_t)(w >> 32) + __popc((uint32_t)w & ((1u << (d & 31)) - 1));
+        slots[pos] = (gnull >> j) & 1 ? null_slot : (int32_t)(grp[j] - grp_min);
       }
     }
   }
+}
+
+struct b2_scan_io_dir {
+  uint64_t* dir;
+  __device__ int64_t get(int64_t i) const { return __popc((uint32_t)dir[i]); }
+  __device__ void put(int64_t i, int64_t v) const { dir[i] = (uint64_t)(uint32_t)dir[i] | ((uint64_t)v << 32); }
+};
+
+__global__ void __launch_bounds__(B2_SCAN_THREADS) b2_star_build_rank_kernel(uint64_t* __restrict__ dir, int64_t nwords) {
+  b2_block_exclusive_scan(b2_scan_io_dir{dir}, nwords);
 }
 
 __global__ void __launch_bounds__(B2_BLOCK)
@@ -358,8 +390,27 @@ __device__ __forceinline__ void b2_star_body(const b2_scan_t& s, const LD& ld, i
   uint32_t live = bits;
   if (kc.valid) live &= b2_valid_bits<R>(kc.valid, ld.row0, bits);
   // all lookups of the batch are issued before the first one is consumed
+  const bool prefetch = aggs.n > 0 && aggs.a[0].col >= 0;
+  int64_t pre[R];   // only read when `prefetch`: otherwise aggregate 0 has no input column, or is absent
   int32_t found[R];
-  if (lk.dense) {
+  if (lk.dense == 2) {
+    // ranked bitmap: every directory word first, then the slot reads for the keys whose bit is set.
+    // The prefetch is issued between the two so that it stays in flight across both round trips.
+    const uint64_t range = (uint64_t)lk.range;
+    uint64_t w[R];
+#pragma unroll
+    for (int j = 0; j < R; ++j) {
+      const uint64_t d = (uint64_t)key[j] - (uint64_t)lk.kmin;
+      w[j] = (((live >> j) & 1) && d < range) ? (uint64_t)b2_ld_keep_i64(reinterpret_cast<const int64_t*>(lk.dir) + (d >> 5)) : 0;
+    }
+    if (prefetch) ld.template load<R>(aggs.a[0].col, live, false, pre);
+#pragma unroll
+    for (int j = 0; j < R; ++j) {
+      const uint32_t b = (uint32_t)((uint64_t)key[j] - (uint64_t)lk.kmin) & 31;
+      const uint32_t bits = (uint32_t)w[j];
+      found[j] = (bits >> b) & 1 ? b2_ld_keep_i32(lk.lookup + (uint32_t)(w[j] >> 32) + __popc(bits & ((1u << b) - 1))) : -1;
+    }
+  } else if (lk.dense) {
     const uint64_t range = (uint64_t)lk.range;
 #pragma unroll
     for (int j = 0; j < R; ++j) {
@@ -373,13 +424,12 @@ __device__ __forceinline__ void b2_star_body(const b2_scan_t& s, const LD& ld, i
       if (((live >> j) & 1) && key[j] != B2_EMPTY_KEY) found[j] = b2_star_lookup(lk, key[j]);
     }
   }
-  const bool prefetch = aggs.n > 0 && aggs.a[0].col >= 0;
-  int64_t pre[R];
-  if (prefetch) ld.template load<R>(aggs.a[0].col, live, false, pre);
+  if (lk.dense != 2 && prefetch) ld.template load<R>(aggs.a[0].col, live, false, pre);
   int64_t slot[R];
 #pragma unroll
   for (int j = 0; j < R; ++j) slot[j] = found[j];
-  b2_apply_aggs<R>(s, ld, aggs.a, aggs.n, st, slot, prefetch ? pre : nullptr);
+  // `pre` is passed as it is, never as a pointer chosen at run time: that would put it in local memory
+  b2_apply_aggs<R>(s, ld, aggs.a, aggs.n, st, slot, pre);
 }
 
 template <bool PIPE>
@@ -597,22 +647,49 @@ int32_t b2_star_build_dense(const b2_col_t* pk, const int32_t* sel, int64_t n_se
   return B2_OK;
 }
 
-int32_t b2_star_build_scan(const b2_scan_t* scan, int32_t pk_col, int32_t grp_col, int64_t pk_min,
-                           int64_t pk_range, int64_t grp_min, int32_t null_slot, int32_t* lookup,
-                           int32_t* d_flags, void* stream) {
+static int32_t b2_star_build_pass(bool fill, const b2_scan_t* scan, int32_t pk_col, int32_t grp_col,
+                                  int64_t pk_min, int64_t pk_range, int64_t grp_min, int32_t null_slot,
+                                  uint64_t* dir, int32_t* slots, int32_t* d_flags, void* stream) {
   int32_t rc = b2_check_scan(scan);
   if (rc) return rc;
-  B2_REQUIRE(lookup && d_flags, "null argument");
   B2_REQUIRE(pk_col >= 0 && pk_col < scan->ncols && grp_col >= 0 && grp_col < scan->ncols, "column out of range");
   B2_REQUIRE(scan->cols[pk_col].dtype == B2_I64 && scan->cols[grp_col].dtype == B2_I64, "dense keys must be int64");
-  B2_REQUIRE(pk_range > 0, "bad range");
+  B2_REQUIRE(pk_range > 0 && pk_range < ((int64_t)1 << 31), "bad range");
   if (scan->n == 0) return B2_OK;
   int64_t nblk = (scan->n + B2_GB_ROWS_PER_BLOCK - 1) / B2_GB_ROWS_PER_BLOCK;
-  int grid = b2_wave_grid(b2_star_build_scan_kernel, B2_BLOCK, nblk);
-  b2_star_build_scan_kernel<<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(*scan, pk_col, grp_col, pk_min, pk_range,
-                                                                          grp_min, null_slot, lookup, d_flags);
+  if (fill) {
+    int grid = b2_wave_grid(b2_star_build_scan_kernel<true>, B2_BLOCK, nblk);
+    b2_star_build_scan_kernel<true><<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(*scan, pk_col, grp_col, pk_min, pk_range,
+                                                                                  grp_min, null_slot, dir, slots, d_flags);
+  } else {
+    int grid = b2_wave_grid(b2_star_build_scan_kernel<false>, B2_BLOCK, nblk);
+    b2_star_build_scan_kernel<false><<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(*scan, pk_col, grp_col, pk_min, pk_range,
+                                                                                   grp_min, null_slot, dir, slots, d_flags);
+  }
   B2_CHECK_LAUNCH("b2_star_build_scan_kernel");
   return B2_OK;
+}
+
+int32_t b2_star_build_mark(const b2_scan_t* scan, int32_t pk_col, int64_t pk_min, int64_t pk_range, uint64_t* dir,
+                           int32_t* d_flags, void* stream) {
+  B2_REQUIRE(dir && d_flags, "null argument");
+  return b2_star_build_pass(false, scan, pk_col, pk_col, pk_min, pk_range, 0, 0, dir, nullptr, d_flags, stream);
+}
+
+int32_t b2_star_build_rank(uint64_t* dir, int64_t pk_range, void* stream) {
+  B2_REQUIRE(dir, "null argument");
+  B2_REQUIRE(pk_range > 0 && pk_range < ((int64_t)1 << 31), "bad range");
+  b2_star_build_rank_kernel<<<1, B2_SCAN_THREADS, 0, (cudaStream_t)stream>>>(dir, (pk_range + 31) / 32);
+  B2_CHECK_LAUNCH("b2_star_build_rank_kernel");
+  return B2_OK;
+}
+
+int32_t b2_star_build_fill(const b2_scan_t* scan, int32_t pk_col, int32_t grp_col, int64_t pk_min,
+                           int64_t pk_range, int64_t grp_min, int32_t null_slot, const uint64_t* dir,
+                           int32_t* slots, void* stream) {
+  B2_REQUIRE(dir && slots, "null argument");
+  return b2_star_build_pass(true, scan, pk_col, grp_col, pk_min, pk_range, grp_min, null_slot,
+                            const_cast<uint64_t*>(dir), slots, nullptr, stream);
 }
 
 int32_t b2_star_build_hash(const b2_col_t* pk, const int32_t* sel, int64_t n_sel, const int32_t* slot_of_row,
@@ -639,7 +716,9 @@ int32_t b2_star_agg(const b2_scan_t* scan, int32_t fk_col, const b2_starlookup_t
   B2_REQUIRE(lk, "null lookup");
   B2_REQUIRE(fk_col >= 0 && fk_col < scan->ncols, "fk column out of range");
   B2_REQUIRE(scan->cols[fk_col].dtype == B2_I64, "fk must be int64");
-  if (lk->dense) B2_REQUIRE(lk->lookup && lk->range > 0, "bad dense lookup");
+  B2_REQUIRE(lk->dense >= 0 && lk->dense <= 2, "bad lookup kind");
+  if (lk->dense == 2) B2_REQUIRE(lk->dir && lk->lookup && lk->range > 0 && lk->range < ((int64_t)1 << 31), "bad bitmap lookup");
+  else if (lk->dense) B2_REQUIRE(lk->lookup && lk->range > 0, "bad dense lookup");
   else B2_REQUIRE(lk->table_keys && lk->table_slots && b2_pow2(lk->cap), "bad hash lookup");
   if (scan->n == 0) return B2_OK;
   b2_pipe_t pp;

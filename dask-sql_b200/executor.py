@@ -1590,8 +1590,8 @@ class PreparedStar:
     re-allocated, per run).  A step of a repeated query then costs the host a few dozen calls instead
     of re-deriving all of it -- at 8 GPUs a step is a few ms of device work, so host time counts.
 
-    One stream, in order: lookup fill -> b2_star_build_scan (every rank that holds dim rows; a 'root' table
-    is followed by one NCCL broadcast of the finished lookup) -> b2_star_agg per fact partition -> merge ->
+    One stream, in order: lookup build (_star_bitmap_build, on every rank that holds dim rows; a 'root'
+    table is followed by one NCCL broadcast of the finished lookup) -> b2_star_agg per fact partition -> merge ->
     compaction.  The lookup buffer is refilled in stream order; with the NVLink peer merge two group
     tables alternate between consecutive executions (peers read a table while its owner has moved on).
     The host issues run k + 2 only after run k has FINISHED (event): at most two executions in flight.
@@ -1646,7 +1646,7 @@ class PreparedStar:
 
     def __init__(self, src, fact, dim, fk_e, pk_e, ge, gexpr0, aggs, fpred, dpred, meta, owner, bcast, sharded, dev):
         self.dev, self.owner, self.bcast, self.sharded = dev, owner, bcast, sharded
-        self.pmin, self.prange, self.gmin, self.grng, self.gnull = meta
+        self.pmin, self.prange, self.gmin, self.grng, self.gnull, dn = meta
         self.nslots = self.grng + 1
         self.gname = src.group_cols[0]
         self.gexpr0 = gexpr0
@@ -1682,13 +1682,13 @@ class PreparedStar:
             self.fact_launch.append((ctx.scan(), fk_slot, D.make_aggs(specs), len(specs), part.n))
             self.keep.append(ctx)
         # ---- reused device buffers
-        # ONE lookup buffer: every run refills it in stream order, after the previous run's scan.  (Two
-        # alternating buffers -- needed while the build ran on its own stream -- would keep 2 x 40 MB of
-        # evict_last lines next to the group tables, more than the whole 50 MB L2, and a step would meet a
-        # lookup that the other buffer's protected lines have displaced.)
-        self.lookup = torch.empty(self.prange + 4, dtype=torch.int32, device=dev)
-        self.lk = L.StarLookup()
-        self.lk.dense, self.lk.lookup, self.lk.kmin, self.lk.range = 1, self.lookup.data_ptr(), self.pmin, self.prange
+        # ONE lookup buffer: every run rebuilds it in stream order, after the previous run's scan.  (Two
+        # alternating buffers would keep both sets of evict_last lines next to the group tables, and a step
+        # would meet a lookup that the other buffer's protected lines have displaced.)
+        self.dn = dn
+        _, self.flags_off, words = _star_bitmap_words(self.prange, dn)
+        self.lookup = torch.empty(words, dtype=torch.int32, device=dev)
+        self.lk = _star_bitmap_lookup(self.lookup, self.pmin, self.prange, dn)
         # group tables: ONE (re-initialised per run) on the NCCL / single-GPU path; enable_peer_merge()
         # replaces it with two in symmetric memory that alternate run by run
         self.tabs = [GroupState(dev, self.nslots, self.plan, need_present=True,
@@ -1827,15 +1827,10 @@ class PreparedStar:
         # nothing to gain: the scan kernels are persistent grids that fill every SM, so the build kernels
         # wait for a whole fact partition anyway, and the extra stream, communicator and events only add
         # cost.)
-        with _Phase("build"):
-            # lookup := -1 everywhere (0xFF bytes), the 4 flag words behind it := 0
-            L.memset(C.c_void_p(buf.data_ptr()), 0xFF, 4 * self.prange, sp)
-            L.memset(C.c_void_p(buf.data_ptr() + 4 * self.prange), 0, 16, sp)
-            for scan, pk_slot, g_slot in self.dim_launch:
-                stats["launches"] += 1
-                L.star_build_scan(C.byref(scan), pk_slot, g_slot, self.pmin, self.prange, self.gmin,
-                                  self.nslots - 1, C.c_void_p(buf.data_ptr()),
-                                  C.c_void_p(buf.data_ptr() + 4 * self.prange), sp)
+        if self.owner:
+            with _Phase("build"):
+                _star_bitmap_build(buf, self.dim_launch, self.pmin, self.prange, self.gmin, self.nslots - 1,
+                                   self.dn, sp)
         if self.bcast:
             with _Phase("bcast"):
                 P.broadcast_(buf, 0)
@@ -1870,7 +1865,7 @@ class PreparedStar:
             return run_aggregate(src, allow_fast=False)
 
         out = _finalize_dense(view, self.gmin, self.gname, self.gexpr0, self.glog, self.plan, self.dev,
-                              key_nullable=self.gnull, check=buf[self.prange:], fallback=general)
+                              key_nullable=self.gnull, check=buf[self.flags_off:], fallback=general)
         done = torch.cuda.Event()
         done.record(main)
         self.free[i] = done
@@ -1881,10 +1876,45 @@ class _NotPreparable(Exception):
     pass
 
 
+def _star_bitmap_words(prange, dn):
+    """int32 offsets within the one buffer of a ranked-bitmap star lookup (include/b200sql.h,
+    b2_star_build_mark): (slots, flags, total).  The directory comes first, two words per 32 keys; the
+    slots hold one entry per set bit, at most one per dim row and one per key; 4 flag words close it.
+    One buffer, so that a 'root' table's lookup crosses to the other ranks in one broadcast."""
+    slots = 2 * ((prange + 31) // 32)
+    flags = slots + min(dn, prange)
+    return slots, flags, flags + 4
+
+
+def _star_bitmap_lookup(buf, pmin, prange, dn):
+    lk = L.StarLookup()
+    lk.dense, lk.dir, lk.kmin, lk.range = 2, buf.data_ptr(), pmin, prange
+    lk.lookup = buf.data_ptr() + 4 * _star_bitmap_words(prange, dn)[0]
+    return lk
+
+
+def _star_bitmap_build(buf, launches, pmin, prange, gmin, null_slot, dn, sp):
+    """The ranked-bitmap lookup from (scan, pk slot, grp slot) of every dim partition, in stream order:
+    zero the directory and flags, mark every partition, rank, fill every partition."""
+    slots_off, flags_off, _ = _star_bitmap_words(prange, dn)
+    base = buf.data_ptr()
+    dirp, slots, flags = C.c_void_p(base), C.c_void_p(base + 4 * slots_off), C.c_void_p(base + 4 * flags_off)
+    L.memset(dirp, 0, 4 * slots_off, sp)
+    L.memset(flags, 0, 16, sp)
+    for scan, pk_slot, _ in launches:
+        stats["launches"] += 1
+        L.star_build_mark(C.byref(scan), pk_slot, pmin, prange, dirp, flags, sp)
+    stats["launches"] += 1
+    L.star_build_rank(dirp, prange, sp)
+    for scan, pk_slot, g_slot in launches:
+        stats["launches"] += 1
+        L.star_build_fill(C.byref(scan), pk_slot, g_slot, pmin, prange, gmin, null_slot, dirp, slots, sp)
+
+
 def _star_dense_fast(src, fact, dim, fk_e, pk_e, gexprs, aggs, fact_pred, dim_pred, sharded, dev) -> Optional[Part]:
     """Star pipeline when the dimension side is a registered table whose join key and (single)
-    group key are dense int64 columns: b2_star_build_scan per dim partition, b2_star_agg per fact
-    partition, one compaction at the end.  Returns None when the shape does not apply or a
+    group key are dense int64 columns: the ranked-bitmap lookup built from the dim partitions
+    (_star_bitmap_build), b2_star_agg per fact partition, one compaction at the end.  Returns None when the shape does not apply or a
     duplicate build key shows up (the general path then takes over)."""
     if len(gexprs) != 1 or not isinstance(dim.source, TableSource) or not isinstance(pk_e, ColRef):
         return None
@@ -1925,35 +1955,35 @@ def _star_dense_fast(src, fact, dim, fk_e, pk_e, gexprs, aggs, fact_pred, dim_pr
     nslots = grng + 1
     if os.environ.get("B200SQL_NO_PREPARED") != "1":
         prep = PreparedStar.get(src, fact, dim, fk_e, pk_e, ge, gexprs[0], aggs, fpred, dpred,
-                                (pmin, prange, gmin, grng, gnull), owner, world > 1 and dist == "root", sharded, dev)
+                                (pmin, prange, gmin, grng, gnull, dn), owner, world > 1 and dist == "root", sharded, dev)
         if prep is not None:
             return prep.run(src)
-    # lookup and the 4 flag words share one buffer: one broadcast carries both
-    buf = torch.full((prange + 4,), -1, dtype=torch.int32, device=dev)
-    lookup, flags = buf[:prange], buf[prange:]
-    flags.zero_()
+    # directory, slots and the 4 flag words share one buffer: one broadcast carries them all
+    _, flags_off, words = _star_bitmap_words(prange, dn)
+    buf = torch.empty(words, dtype=torch.int32, device=dev)
+    flags = buf[flags_off:]
     with _Phase("build"):
         if owner:
             needed: Set[str] = {pk_e.name, ge.name}
             for p in dpred:
                 p.refs(needed)
+            launches, keep = [], []
             for part in materialize(dim.source, needed):
                 if part.n == 0:
                     continue
                 ctx = ScanCtx(part, dpred)
                 pk_slot, g_slot = ctx.slot(pk_e), ctx.slot(ge)     # slots first: scan() snapshots the columns
-                stats["launches"] += 1
-                L.star_build_scan(C.byref(ctx.scan()), pk_slot, g_slot, pmin, prange, gmin, nslots - 1,
-                                  D.ptr(lookup), D.ptr(flags), D.stream_ptr())
+                launches.append((ctx.scan(), pk_slot, g_slot))
+                keep.append(ctx)
+            _star_bitmap_build(buf, launches, pmin, prange, gmin, nslots - 1, dn, D.stream_ptr())
     if world > 1 and dist == "root":
-        # the build side crosses NVLink as the finished 4-byte-per-key lookup, not as its columns
+        # the build side crosses NVLink as the finished lookup (directory + slots), not as its columns
         with _Phase("bcast"):
             P.broadcast_(buf, 0)
     plan = AggPlan([(E.substitute(e, fact.exprs) if e is not None else None, o, f) for e, o, f in aggs],
                    _nullable_fn(fact, sharded))
     gs = GroupState(dev, nslots, plan, need_present=True, alloc=_padded_slots(nslots, sharded))
-    lk = L.StarLookup()
-    lk.dense, lk.lookup, lk.kmin, lk.range = 1, lookup.data_ptr(), pmin, prange
+    lk = _star_bitmap_lookup(buf, pmin, prange, dn)
     needed = set(fk_e.refs())
     for ka in plan.kaggs:
         ka.expr.refs(needed)

@@ -511,13 +511,22 @@ int32_t b2_dense_slots(const b2_col_t* key, int64_t n, int64_t kmin, int32_t nul
 int32_t b2_star_build_dense(const b2_col_t* pk, const int32_t* sel, int64_t n_sel,
                             const int32_t* slot_of_row, int64_t kmin, int64_t range,
                             int32_t* lookup, int32_t* d_flags, void* stream);
-/* The same lookup straight from the UNFILTERED build partition when join key and group key are both
- * dense int64: rows of `scan` passing its terms write lookup[pk-pk_min] = grp-grp_min (NULL grp ->
- * null_slot, NULL pk skipped).  Fuses table_scan.py:80-119 (dim filter) into the build; nothing is
- * materialised.  Call once per build partition; d_flags[0] = 1 on duplicate pk. */
-int32_t b2_star_build_scan(const b2_scan_t* scan, int32_t pk_col, int32_t grp_col, int64_t pk_min,
-                           int64_t pk_range, int64_t grp_min, int32_t null_slot, int32_t* lookup,
-                           int32_t* d_flags, void* stream);
+/* A ranked-bitmap lookup (b2_starlookup_t.dense == 2) straight from the UNFILTERED build partitions
+ * when join key and group key are both dense int64.  Fuses table_scan.py:80-119 (dim filter) into the
+ * build; nothing is materialised.  Layout:
+ *   dir   = uint64[(pk_range + 31) / 32]: bits (low half) = one bit per key of [pk_min, pk_min + pk_range)
+ *           whose build row passes the terms and has a non-NULL key; rank (high half) = set bits in all
+ *           earlier words;
+ *   slots = int32[min(build rows, pk_range)]: one entry per set bit in key order, grp - grp_min
+ *           (NULL grp -> null_slot).
+ * In stream order: zero dir; b2_star_build_mark on every build partition (d_flags[0] = 1 on a duplicate
+ * pk among the rows that pass); b2_star_build_rank once; b2_star_build_fill on every build partition. */
+int32_t b2_star_build_mark(const b2_scan_t* scan, int32_t pk_col, int64_t pk_min, int64_t pk_range,
+                           uint64_t* dir, int32_t* d_flags, void* stream);
+int32_t b2_star_build_rank(uint64_t* dir, int64_t pk_range, void* stream);
+int32_t b2_star_build_fill(const b2_scan_t* scan, int32_t pk_col, int32_t grp_col, int64_t pk_min,
+                           int64_t pk_range, int64_t grp_min, int32_t null_slot, const uint64_t* dir,
+                           int32_t* slots, void* stream);
 /* Hash variant: table_keys = int64[cap] pre-filled with B2_EMPTY_KEY, table_slots = int32[cap].
  * d_flags[0] = 1 on duplicate pk, d_flags[1] = 1 on overflow. */
 int32_t b2_star_build_hash(const b2_col_t* pk, const int32_t* sel, int64_t n_sel,
@@ -525,14 +534,15 @@ int32_t b2_star_build_hash(const b2_col_t* pk, const int32_t* sel, int64_t n_sel
                            int64_t cap, int32_t* d_flags, void* stream);
 
 typedef struct b2_starlookup {
-  int32_t dense;
+  int32_t dense;           /* 0: hash table, 1: int32 per key, 2: ranked bitmap (b2_star_build_mark) */
   int32_t pad_;
-  const int32_t* lookup;   /* dense: int32[range], -1 = no partner */
+  const int32_t* lookup;   /* 1: int32[range], -1 = no partner; 2: the slots array */
   int64_t kmin;
   int64_t range;
   const int64_t* table_keys;  /* hash */
   const int32_t* table_slots;
   int64_t cap;
+  const uint64_t* dir;     /* 2: the directory */
 } b2_starlookup_t;
 
 /* One pass over the probe (fact) partition: predicate -> key lookup -> aggregate into the
