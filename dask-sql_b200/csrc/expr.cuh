@@ -100,10 +100,13 @@ b2_expr_kernel(const __grid_constant__ b2_prog_t prog, const __grid_constant__ b
             if (b == 0) rn = true;
             else if (b == -1) r = (int64_t)(0ULL - (uint64_t)a);
             else r = a / b;  // C++ '/' truncates toward zero = SQL semantics
-          } else if (op == B2_OP_MOD_I) {
+          } else if (op == B2_OP_MOD_I) {  // floored, like NumPy / Python: the result takes b's sign
             if (b == 0) rn = true;
             else if (b == -1) r = 0;
-            else r = a % b;
+            else {
+              r = a % b;
+              if (r != 0 && (r ^ b) < 0) r += b;
+            }
           } else if (op == B2_OP_ADD_F) r = __double_as_longlong(__longlong_as_double(a) + __longlong_as_double(b));
           else if (op == B2_OP_SUB_F) r = __double_as_longlong(__longlong_as_double(a) - __longlong_as_double(b));
           else if (op == B2_OP_MUL_F) r = __double_as_longlong(__longlong_as_double(a) * __longlong_as_double(b));

@@ -12,6 +12,7 @@ import numpy as np
 import torch
 
 from . import _lib as L
+from .expr import int_literal_is_exact
 
 I64, F64, U8 = L.I64, L.F64, L.U8
 _TORCH_DTYPE = {I64: torch.int64, F64: torch.float64, U8: torch.uint8}
@@ -243,10 +244,8 @@ def make_scan(cols: Sequence[DeviceColumn], terms: Sequence[TermSpec], n: Option
             continue
         if cd == F64:
             tm.lit_f = float(lit)
-        elif isinstance(lit, (float, np.floating)) and not float(lit).is_integer():
-            tm.as_f64, tm.lit_f = 1, float(lit)
-        elif isinstance(lit, (float, np.floating)) and abs(float(lit)) >= 2 ** 63:
-            tm.as_f64, tm.lit_f = 1, float(lit)
+        elif isinstance(lit, (float, np.floating)) and not int_literal_is_exact(float(lit)):
+            tm.as_f64, tm.lit_f = 1, float(lit)     # compares in float64, see expr.F64_EXACT_INT
         else:
             tm.lit_i = int(lit)
     return s

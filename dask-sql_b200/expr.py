@@ -17,6 +17,16 @@ _DT_NAME = {I64: "int64", F64: "float64", U8: "bool"}
 _CMP = {"eq": L.EQ, "ne": L.NE, "lt": L.LT, "le": L.LE, "gt": L.GT, "ge": L.GE}
 _FLIP = {"eq": "eq", "ne": "ne", "lt": "gt", "le": "ge", "gt": "lt", "ge": "le"}
 
+# An int64 column compared with a float literal compares in float64 (NumPy, and SQL's implicit cast to
+# DOUBLE).  An integer-valued literal may become an exact int64 comparison only while |lit| < 2^53: there
+# float(x) <op> lit  <=>  x <op> int(lit)  for every int64 x.  From 2^53 on float(x) rounds
+# (float(2^53 + 1) == 2^53), so such a term keeps comparing in float64 (b2_term_t.as_f64).
+F64_EXACT_INT = 2 ** 53
+
+
+def int_literal_is_exact(lit: float) -> bool:
+    return lit.is_integer() and abs(lit) < F64_EXACT_INT
+
 
 class Expr:
     dtype: int = I64
@@ -203,7 +213,7 @@ def as_term(e: Expr) -> Optional[Tuple[str, int, object]]:
             lit = b.value
             if as_f or col.dtype == F64:
                 lit = float(lit)
-                if col.dtype == I64 and lit.is_integer() and abs(lit) < 2 ** 62:
+                if col.dtype == I64 and int_literal_is_exact(lit):
                     lit = int(lit)
             return col.name, _CMP[op], lit
         return None

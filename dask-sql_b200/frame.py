@@ -148,6 +148,7 @@ class LazySeries:
     def __truediv__(self, o): return self._bin("truediv", o)
     def __rtruediv__(self, o): return self._bin("truediv", o, True)
     def __mod__(self, o): return self._bin("mod", o)
+    def __rmod__(self, o): return self._bin("mod", o, True)
     def __gt__(self, o): return self._bin("gt", o)
     def __ge__(self, o): return self._bin("ge", o)
     def __lt__(self, o): return self._bin("lt", o)

@@ -84,6 +84,14 @@ def _divide(a, b, rex):
     return int(np.trunc(a / b))
 
 
+def _modulo(a, b):
+    """SQL '%': floored like the reference's da.mod (NumPy) and the B2_OP_MOD_I kernel, -7 % 3 = 2;
+    a zero divisor is NULL, for scalars as in _divide and in the kernel."""
+    if is_frame(a) or is_frame(b):
+        return a % b
+    return None if b == 0 else a % b
+
+
 def _unary(on_series, on_scalar):
     def run(args, rex):
         (x,) = args
@@ -176,7 +184,7 @@ OPERATORS.update({
     "+": _left_fold(_strict(operator.add), alone=lambda x: x),
     "-": _left_fold(_strict(operator.sub), alone=lambda x: None if x is None else -x),
     "*": _left_fold(_strict(operator.mul)),
-    "%": _left_fold(_strict(operator.mod)),
+    "%": _left_fold(_strict(_modulo)),
     "/": _left_fold(_divide),
     "negative": _unary(operator.neg, lambda x: None if x is None else -x),
     "abs": _unary(lambda s: s.abs(), lambda x: None if x is None else abs(x)),

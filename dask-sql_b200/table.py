@@ -440,6 +440,10 @@ class ParquetTable(DeviceTable):
                 rule = rules.get(op)
                 if st is None or rule is None:
                     continue
+                if isinstance(lit, float) and isinstance(st["min"], int):
+                    # the kernel compares an int column with a float literal in float64, where 2^53 + 1
+                    # equals 2^53 (expr.F64_EXACT_INT); Python's exact int/float comparison would prune it
+                    st = dict(st, min=float(st["min"]), max=float(st["max"]))
                 try:
                     if rule(st, lit):
                         dead = True

@@ -147,14 +147,14 @@ typedef struct b2_prog {
 #define B2_OP_CONST_F   2
 #define B2_OP_CONST_NULL 3
 #define B2_OP_I2F       4
-#define B2_OP_F2I       5   /* truncate toward zero */
+#define B2_OP_F2I       5   /* truncate toward zero; NaN -> NULL; saturates at +-inf and |x| >= 2^63 */
 #define B2_OP_ADD_I    10
 #define B2_OP_SUB_I    11
 #define B2_OP_MUL_I    12
 #define B2_OP_DIV_I    13   /* SQL truncated division (call.py:165-189); x/0 -> NULL */
 #define B2_OP_NEG_I    14
 #define B2_OP_ABS_I    15
-#define B2_OP_MOD_I    16
+#define B2_OP_MOD_I    16   /* floored (NumPy / Python '%'): -7 % 3 = 2, 7 % -3 = -2; x%0 -> NULL */
 #define B2_OP_ADD_F    20
 #define B2_OP_SUB_F    21
 #define B2_OP_MUL_F    22

@@ -459,3 +459,60 @@ def test_lazy_parquet_pushdown_end_to_end(c, tmp_path):
                 return_futures=False)
     e = df[df.a < 5000].merge(pd.DataFrame({"k": np.arange(40), "w": np.arange(40) * 2.0}), on="k")
     assert_same(got, e.groupby("w").agg(s=("v", "sum")).reset_index(), ["s"])
+
+
+def test_modulo_is_floored_for_columns_and_constants(c):
+    """SQL '%' is floored (the reference's da.mod, NumPy): the kernel on a column and the host's constant
+    fold agree, -7 % 3 = 2; a zero divisor is NULL on both (DESIGN.md section 6).  Not sqlite: its % truncates."""
+    a = np.array([-7, 7, -6, 5, 0, -1, 1, 2 ** 62 + 1, -(2 ** 63), 2 ** 63 - 1, 0], np.int64)
+    null = np.zeros(len(a), bool)
+    null[[4, 10]] = True
+    df = pd.DataFrame({"a": pd.arrays.IntegerArray(a, null)})
+    c.create_table("t", df, npartitions=2)
+    got = c.sql("SELECT a, a % 3 AS m3, a % -3 AS mm3, -7 % a AS r, -7 % 3 AS k, 7 % -3 AS k2, a % 0 AS z, "
+                "7 % 0 AS z2 FROM t", return_futures=False)
+    av = np.where(null, 0, a)
+
+    def col(v, null=null):
+        return pd.array(np.where(null, None, v).tolist(), dtype="Int64")
+
+    r = col(np.mod(-7, np.where(av == 0, 1, av)), null | (av == 0))
+    exp = pd.DataFrame({"a": df["a"], "m3": col(np.mod(av, 3)), "mm3": col(np.mod(av, -3)), "r": r, "k": 2, "k2": -2,
+                        "z": pd.array([None] * len(a), dtype="Int64"), "z2": pd.array([None] * len(a), dtype="Int64")})
+    assert_same(got, exp)
+    got = c.sql("SELECT a FROM t WHERE a % 3 = -7 % 3", return_futures=False)
+    assert sorted(got["a"].tolist()) == sorted(int(x) for x, n in zip(a, null) if not n and x % 3 == 2)
+
+
+def test_int_column_against_float_literal_at_2_53(c):
+    """x = 9007199254740992.0 (2^53) compares in float64, where 2^53 + 1 rounds to 2^53, both as a lone
+    conjunct (a kernel term) and inside an OR (the expression interpreter)"""
+    x = np.array([2 ** 53 - 1, 2 ** 53, 2 ** 53 + 1, -(2 ** 53) - 1, 5, 2 ** 53 + 2], np.int64)
+    y = pd.array([1, None, 2, 3, 4, 5], dtype="Int64")
+    c.create_table("t", pd.DataFrame({"x": x, "y": y}))
+    for lit, op in (("9007199254740992.0", "="), ("-9007199254740992.0", "="), ("9007199254740992.0", "<>"),
+                    ("9007199254740992.0", "<"), ("9007199254740992.0", ">="), ("9007199254740993.0", ">")):
+        hit = {"=": np.equal, "<>": np.not_equal, "<": np.less, ">=": np.greater_equal,
+               ">": np.greater}[op](x.astype(np.float64), float(lit))
+        alone = c.sql(f"SELECT x FROM t WHERE x {op} {lit}", return_futures=False)
+        inside = c.sql(f"SELECT x FROM t WHERE x {op} {lit} OR y IS NULL", return_futures=False)
+        assert sorted(alone["x"].tolist()) == sorted(x[hit].tolist()), (op, lit)
+        assert sorted(inside["x"].tolist()) == sorted(x[hit | y.isna()].tolist()), (op, lit)
+
+
+def test_order_by_float_edges(c):
+    """ORDER BY over ±inf, ±0.0, subnormals, NaN and NULL: NaN sorts with the NULLs, -0.0 ties with 0.0"""
+    rng = np.random.default_rng(12)
+    n = 20_003
+    f = rng.choice(np.array([np.inf, -np.inf, 0.0, -0.0, np.nan, 5e-324, -5e-324, 1.5, -1.5]), n)
+    df = pd.DataFrame({"i": np.arange(n), "f": f})
+    c.create_table("t", df, npartitions=3)
+    for sql, asc, na in (("ORDER BY f", True, "last"), ("ORDER BY f DESC", False, "first"),
+                         ("ORDER BY f NULLS FIRST", True, "first"), ("ORDER BY f DESC NULLS LAST", False, "last")):
+        got = c.sql(f"SELECT i, f FROM t {sql}", return_futures=False)
+        exp = df.sort_values("f", ascending=asc, na_position=na, kind="stable")
+        np.testing.assert_array_equal(got["f"].to_numpy(), exp["f"].to_numpy(), err_msg=sql)   # -0.0 == 0.0 here
+        assert sorted(got["i"].tolist()) == list(range(n)), sql
+    got = c.sql("SELECT i, f FROM t ORDER BY f, i DESC", return_futures=False)
+    exp = df.assign(z=df.f + 0.0).sort_values(["z", "i"], ascending=[True, False], na_position="last", kind="stable")
+    np.testing.assert_array_equal(got["i"].to_numpy(), exp["i"].to_numpy())                 # ±0.0 tie: i decides
