@@ -516,3 +516,138 @@ def test_order_by_float_edges(c):
     got = c.sql("SELECT i, f FROM t ORDER BY f, i DESC", return_futures=False)
     exp = df.assign(z=df.f + 0.0).sort_values(["z", "i"], ascending=[True, False], na_position="last", kind="stable")
     np.testing.assert_array_equal(got["i"].to_numpy(), exp["i"].to_numpy())                 # ±0.0 tie: i decides
+
+
+# ---- group-by edges: expected values from NumPy / fractions, not from pandas' summation ----------------------
+def _groups(got, key):
+    """{key (NaN -> None): row} of a GROUP BY result"""
+    out = {}
+    for r in got.to_dict("records"):            # per-column types: an int64 key stays an int
+        k = r[key]
+        out[None if pd.isna(k) else k] = r
+    return out
+
+
+def test_groupby_double_key_edges(c):
+    """-0.0 and +0.0 are one group, NaN (any payload) and NULL are the NULL group, +-inf are groups of their own"""
+    nan2 = np.array([0x7FF8000000000001], np.int64).view(np.float64)[0]
+    keys = np.array([0.0, -0.0, np.nan, nan2, np.inf, -np.inf, 1.5, -0.0, np.inf, 2.5])
+    null = np.zeros(len(keys), bool)
+    null[9] = True                                  # a NULL next to the two NaN payloads
+    rng = np.random.default_rng(1)
+    reps = 3001
+    df = pd.DataFrame({"f": np.tile(keys, reps), "v": rng.integers(-100, 100, len(keys) * reps)})
+    df.loc[np.tile(null, reps), "f"] = None
+    c.create_table("t", df, npartitions=3)
+    got = _groups(c.sql("SELECT f, COUNT(*) AS n, SUM(v) AS s FROM t GROUP BY f", return_futures=False), "f")
+    kk = np.tile(keys, reps)
+    ident = np.where(np.isnan(kk) | np.tile(null, reps), np.nan, kk + 0.0)
+    exp = {}
+    for k in (0.0, np.inf, -np.inf, 1.5, None):
+        sel = np.isnan(ident) if k is None else ident == k
+        exp[k] = (int(sel.sum()), int(df.v.to_numpy()[sel].sum()))
+    assert set(got) == set(exp), sorted(map(str, got))
+    for k, (n, s) in exp.items():
+        assert (got[k]["n"], got[k]["s"]) == (n, s), k
+
+
+def test_groupby_boolean_key_with_nulls(c):
+    rng = np.random.default_rng(2)
+    n = 50_003
+    b = rng.integers(0, 2, n).astype(bool)
+    null = rng.random(n) < 0.1
+    df = pd.DataFrame({"b": pd.array(np.where(null, None, b).tolist(), dtype="boolean"), "v": rng.integers(-9, 9, n)})
+    c.create_table("t", df, npartitions=2)
+    got = _groups(c.sql("SELECT b, COUNT(*) AS n, SUM(v) AS s FROM t GROUP BY b", return_futures=False), "b")
+    v = df.v.to_numpy()
+    exp = {True: ~null & b, False: ~null & ~b, None: null}
+    assert set(got) == set(exp)
+    for k, sel in exp.items():
+        assert (got[k]["n"], got[k]["s"]) == (sel.sum(), v[sel].sum()), k
+
+
+def test_groupby_bigint_extreme_keys_sum_wraps_and_avg_near_2_62(c):
+    """keys INT64_MIN and INT64_MAX; per-group SUM wraps (two's complement), AVG near 2^62 is within the
+    float-sum bound of the exact mean"""
+    from fractions import Fraction
+    rng = np.random.default_rng(3)
+    n = 30_001
+    k = rng.choice(np.array([-(2 ** 63), 2 ** 63 - 1, 0, 5], np.int64), n)
+    v = (2 ** 62 + rng.integers(-2 ** 40, 2 ** 40, n)).astype(np.int64)
+    c.create_table("t", pd.DataFrame({"k": k, "v": v}), npartitions=3)
+    got = _groups(c.sql("SELECT k, SUM(v) AS s, AVG(v) AS m, COUNT(*) AS n FROM t GROUP BY k", return_futures=False), "k")
+    assert set(got) == {-(2 ** 63), 2 ** 63 - 1, 0, 5}
+    for key, r in got.items():
+        vs = [int(x) for x in v[k == key]]
+        wrapped = (sum(vs) + 2 ** 63) % 2 ** 64 - 2 ** 63
+        assert int(r["s"]) == wrapped and int(r["n"]) == len(vs), key
+        exact = Fraction(sum(vs), len(vs))
+        assert abs(Fraction(float(r["m"])) - exact) <= (len(vs) + 2) * 2.0 ** -53 * exact, key
+
+
+def test_groupby_min_max_of_signed_zeros_infinities_and_subnormals(c):
+    """MIN / MAX compare the order-preserving image: MIN{-0.0, +0.0} = -0.0 and MAX = +0.0, whatever came first"""
+    groups = {1: [0.0, -0.0], 2: [-0.0, 0.0], 3: [5e-324, -5e-324, 0.0], 4: [np.inf, -np.inf, 1.0],
+              5: [np.nan, -0.0, None], 6: [None, None]}
+    rows = [(k, x) for k, xs in groups.items() for x in xs]
+    df = pd.DataFrame({"k": [r[0] for r in rows], "x": pd.array([r[1] for r in rows], dtype="Float64")})
+    df["x"] = df["x"].astype("float64")
+    c.create_table("t", df, npartitions=2)
+    got = _groups(c.sql("SELECT k, MIN(x) AS lo, MAX(x) AS hi FROM t GROUP BY k", return_futures=False), "k")
+    exp = {1: (-0.0, 0.0), 2: (-0.0, 0.0), 3: (-5e-324, 5e-324), 4: (-np.inf, np.inf), 5: (-0.0, -0.0), 6: (None, None)}
+    for k, (lo, hi) in exp.items():
+        for name, e in (("lo", lo), ("hi", hi)):
+            g = got[k][name]
+            if e is None:
+                assert pd.isna(g), (k, name, g)
+            else:
+                assert g == e and np.signbit(g) == np.signbit(e), (k, name, g, e)
+
+
+def test_groupby_variance_against_the_exact_two_pass_value(c):
+    """VAR_SAMP / STDDEV on N(1e9, 1) with groups of one and two rows and NULLs, against the exact variance"""
+    from fractions import Fraction
+    rng = np.random.default_rng(4)
+    n = 20_000
+    k = rng.integers(0, 20, n)
+    k[:3] = [100, 101, 101]                       # a group of one row and one of two
+    x = 1e9 + rng.normal(0, 1, n)
+    x[rng.random(n) < 0.05] = np.nan
+    x[:3] = [1e9 + 0.5, 1e9 + 0.25, 1e9 - 0.75]
+    df = pd.DataFrame({"k": k, "x": x})
+    c.create_table("t", df, npartitions=3)
+    got = _groups(c.sql("SELECT k, VAR_SAMP(x) AS v, STDDEV(x) AS s FROM t GROUP BY k", return_futures=False), "k")
+    for key, r in got.items():
+        xs = [Fraction(float(a)) for a in x[(k == key) & ~np.isnan(x)]]
+        if len(xs) < 2:
+            assert pd.isna(r["v"]) and pd.isna(r["s"]), key
+            continue
+        mean = sum(xs) / len(xs)
+        var = float(sum((a - mean) ** 2 for a in xs) / (len(xs) - 1))
+        np.testing.assert_allclose([r["v"], r["s"]], [var, np.sqrt(var)], rtol=1e-9, err_msg=str(key))
+
+
+def test_groupby_skewed_key_whose_hottest_key_is_filtered_out(c, monkeypatch):
+    """Zipf keys under the heavy-hitter kernel: the hottest key is sampled (from the unfiltered column) but every
+    one of its rows fails the WHERE clause, and the never-NULL float SUM is the group's only existence mark:
+    the group must not appear"""
+    from dask_sql_b200 import executor
+    monkeypatch.setenv("B200SQL_SKEW", "hot")
+    rng = np.random.default_rng(5)
+    n = 400_003
+    k = np.minimum(rng.zipf(1.2, n), 5000).astype(np.int64)
+    f = rng.integers(-1, 2 ** 10, n) * 2.0 ** -4
+    f[k == 1] = -1.0                               # key 1 holds ~1/3 of the rows, all filtered
+    v = rng.integers(-2 ** 10, 2 ** 10, n) * 2.0 ** -8
+    c.create_table("t", pd.DataFrame({"k": k, "f": f, "v": v}), npartitions=2)
+    before = executor.stats.get("grouped_groupby", 0)
+    got = _groups(c.sql("SELECT k, SUM(v) AS s FROM t WHERE f >= 0 GROUP BY k", return_futures=False), "k")
+    assert executor.stats.get("grouped_groupby", 0) > before, "the skew path did not run"
+    keep = f >= 0
+    assert 1 not in got
+    assert set(got) == set(np.unique(k[keep]).tolist())
+    sums = {}
+    for key, val in zip(k[keep].tolist(), v[keep].tolist()):
+        sums[key] = sums.get(key, 0.0) + val       # dyadic values: every order gives the same sum
+    for key, r in got.items():
+        assert r["s"] == sums[key], key
