@@ -16,7 +16,7 @@ COL_SENTINEL = 1
 MAX_COLS, MAX_TERMS, MAX_AGGS, MAX_KEYS, MAX_GATHER, MAX_PROG = 16, 8, 8, 4, 8, 64
 TILE = 4096
 EQ, NE, LT, LE, GT, GE, IS_NULL, IS_NOT_NULL, IS_TRUE = range(9)
-AGG_SUM, AGG_SUMF, AGG_MIN, AGG_MAX, AGG_COUNT = range(5)
+AGG_SUM, AGG_SUMF, AGG_MIN, AGG_MAX, AGG_COUNT, AGG_AND, AGG_OR, AGG_XOR = range(8)
 JOIN_INNER, JOIN_LEFT, JOIN_SEMI, JOIN_ANTI = range(4)
 EMPTY_KEY = -(1 << 63)
 
@@ -79,7 +79,7 @@ class StarLookup(C.Structure):
 
 
 MAX_PEERS, PEER_MAX_ARRAYS = 16, 2 * MAX_AGGS + 1
-PEER_SUM_F64, PEER_SUM_I64, PEER_MIN_I64, PEER_MAX_I64 = range(4)
+PEER_SUM_F64, PEER_SUM_I64, PEER_MIN_I64, PEER_MAX_I64, PEER_AND_I64, PEER_OR_I64, PEER_XOR_I64 = range(7)
 PEER_PRESENT_ROWS, PEER_PRESENT_INDICATOR, PEER_PRESENT_BITMAP = 1, 2, 3
 
 
@@ -95,6 +95,12 @@ class PeerMerge(C.Structure):
 assert C.sizeof(Col) == 24 and C.sizeof(Term) == 32 and C.sizeof(Scan) == 656
 assert C.sizeof(AggState) == 152 and C.sizeof(Instr) == 24 and C.sizeof(Prog) == 1544
 assert C.sizeof(JoinTable) == 152 and C.sizeof(StarLookup) == 64 and C.sizeof(PeerMerge) == 544
+
+
+def agg_identity(op):
+    """Initial value of an int64 accumulator of aggregate `op` (the b2_aggstate_t contract): the value that
+    leaves any input unchanged.  Float SUM / SUMF accumulators start at +0.0, whose bits are this 0 too."""
+    return {AGG_MIN: (1 << 63) - 1, AGG_MAX: -(1 << 63), AGG_AND: -1}.get(op, 0)
 
 
 class B200SqlError(RuntimeError):
@@ -178,7 +184,7 @@ _SIGS = {
     "b2_range_partition": [C.POINTER(Scan), C.c_int32, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
                            C.POINTER(C.c_int32), _P, C.POINTER(_P), _P, _P],
     "b2_iota": [_P, C.c_int64, _P],
-    "b2_bitmap_or": [_P, _P, C.c_int64, _P],
+    "b2_bitwise_combine": [_P, _P, C.c_int64, C.c_int32, _P],
     "b2_peer_merge": [C.POINTER(PeerMerge), _P],
     "b2_sort_by": [C.POINTER(Col), C.c_int64, C.c_int32, C.c_int32, _P, _P, _P],
     "b2_dense_slots": [C.POINTER(Col), C.c_int64, C.c_int64, C.c_int32, _P, _P],
@@ -266,7 +272,7 @@ range_partition_scan = _wrap("b2_range_partition_scan")
 range_partition_scatter = _wrap("b2_range_partition_scatter")
 range_partition_ws_bytes = _lib.b2_range_partition_ws_bytes
 iota = _wrap("b2_iota")
-bitmap_or = _wrap("b2_bitmap_or")
+bitwise_combine = _wrap("b2_bitwise_combine")
 peer_merge = _wrap("b2_peer_merge")
 sort_by = _wrap("b2_sort_by")
 _lib.b2_sort_ws_bytes.restype = C.c_int64

@@ -414,7 +414,11 @@ __device__ __forceinline__ uint32_t b2_eval_terms(const b2_scan_t& s, int64_t ro
 #define B2_K_MIN_F   5   // ordered-int64 image
 #define B2_K_MAX_F   6
 #define B2_K_NONE    7   // COUNT only
+#define B2_K_AND     8   // bitwise, one kind for int64 and U8 (0/1) inputs alike
+#define B2_K_OR      9
+#define B2_K_XOR    10
 
+template <bool BITS = true>   // false: the caller's kernel instance has no bitwise aggregate
 __device__ __forceinline__ int b2_agg_kind(int op, int dtype) {
   const bool f = dtype == B2_F64;
   switch (op) {
@@ -422,6 +426,9 @@ __device__ __forceinline__ int b2_agg_kind(int op, int dtype) {
     case B2_AGG_SUMF: return f ? B2_K_SUM_F : B2_K_SUMF_I;
     case B2_AGG_MIN: return f ? B2_K_MIN_F : B2_K_MIN_I;
     case B2_AGG_MAX: return f ? B2_K_MAX_F : B2_K_MAX_I;
+    case B2_AGG_AND: return BITS ? B2_K_AND : B2_K_NONE;
+    case B2_AGG_OR: return BITS ? B2_K_OR : B2_K_NONE;
+    case B2_AGG_XOR: return BITS ? B2_K_XOR : B2_K_NONE;
     default: return B2_K_NONE;
   }
 }
@@ -438,6 +445,10 @@ __device__ __forceinline__ void b2_atomic_k(void* acc, int64_t slot, int64_t raw
   else if (KIND == B2_K_MAX_I) atomicMax(reinterpret_cast<long long*>(acc) + slot, (long long)raw);
   else if (KIND == B2_K_MIN_F) atomicMin(reinterpret_cast<long long*>(acc) + slot, (long long)b2_ordered_from_bits(raw));
   else if (KIND == B2_K_MAX_F) atomicMax(reinterpret_cast<long long*>(acc) + slot, (long long)b2_ordered_from_bits(raw));
+  // one fire-and-forget REDG.E.{AND,OR,XOR}.64 each, like the SUM's REDG.E.ADD.64
+  else if (KIND == B2_K_AND) atomicAnd(reinterpret_cast<unsigned long long*>(acc) + slot, (unsigned long long)raw);
+  else if (KIND == B2_K_OR) atomicOr(reinterpret_cast<unsigned long long*>(acc) + slot, (unsigned long long)raw);
+  else if (KIND == B2_K_XOR) atomicXor(reinterpret_cast<unsigned long long*>(acc) + slot, (unsigned long long)raw);
 }
 
 template <int R, int KIND, bool CNT>
@@ -521,6 +532,9 @@ __device__ __forceinline__ void b2_apply_aggs(const b2_scan_t& s, const LD& ld, 
       case B2_K_MAX_I: b2_atomic_batch<R, B2_K_MAX_I>(acc, cnt, slot, raw, ok); break;
       case B2_K_MIN_F: b2_atomic_batch<R, B2_K_MIN_F>(acc, cnt, slot, raw, ok); break;
       case B2_K_MAX_F: b2_atomic_batch<R, B2_K_MAX_F>(acc, cnt, slot, raw, ok); break;
+      case B2_K_AND: b2_atomic_batch<R, B2_K_AND>(acc, cnt, slot, raw, ok); break;
+      case B2_K_OR: b2_atomic_batch<R, B2_K_OR>(acc, cnt, slot, raw, ok); break;
+      case B2_K_XOR: b2_atomic_batch<R, B2_K_XOR>(acc, cnt, slot, raw, ok); break;
       default: b2_atomic_batch<R, B2_K_NONE>(acc, cnt, slot, raw, ok); break;
     }
   }

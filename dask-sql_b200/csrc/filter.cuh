@@ -17,7 +17,9 @@ struct b2_partial {
   int64_t cnt[B2_MAX_AGGS];
 };
 
+template <bool BITS = true>   // false: the caller has no bitwise aggregate
 __device__ __forceinline__ int64_t b2_combine(int op, int dtype, int64_t a, int64_t b) {
+  if (BITS && op >= B2_AGG_AND) return op == B2_AGG_AND ? a & b : op == B2_AGG_OR ? a | b : a ^ b;
   switch (op) {
     case B2_AGG_SUM:
       if (dtype == B2_F64) return __double_as_longlong(__longlong_as_double(a) + __longlong_as_double(b));
@@ -29,9 +31,11 @@ __device__ __forceinline__ int64_t b2_combine(int op, int dtype, int64_t a, int6
     default: return 0;
   }
 }
+template <bool BITS = true>
 __device__ __forceinline__ int64_t b2_identity(int op) {
   if (op == B2_AGG_MIN) return LLONG_MAX;
   if (op == B2_AGG_MAX) return LLONG_MIN;
+  if (BITS && op == B2_AGG_AND) return -1;
   return 0;  // +0.0 has the same bit pattern
 }
 
@@ -48,13 +52,18 @@ __device__ __forceinline__ int64_t b2_fold_batch(int64_t acc, const int64_t (&ra
     else if (KIND == B2_K_MAX_I) acc = raw[j] > acc ? raw[j] : acc;
     else if (KIND == B2_K_MIN_F) { const int64_t v = b2_ordered_from_bits(raw[j]); acc = v < acc ? v : acc; }
     else if (KIND == B2_K_MAX_F) { const int64_t v = b2_ordered_from_bits(raw[j]); acc = v > acc ? v : acc; }
+    else if (KIND == B2_K_AND) acc &= raw[j];
+    else if (KIND == B2_K_OR) acc |= raw[j];
+    else if (KIND == B2_K_XOR) acc ^= raw[j];
   }
   return acc;
 }
 
 // Accumulators live in shared memory, one slot per (aggregate, thread): the aggregate loop is a
 // run-time loop (no 8-way unrolled register file), the kind switch sits outside the row loop.
-template <int R, class LD>
+// BITS: the instance that also folds AND / OR / XOR.  Those cases live in a kernel instance of their own:
+// inlined into the one every other query runs, they made C1 (a SUM) 4 % slower on H100.
+template <int R, bool BITS, class LD>
 __device__ __forceinline__ void b2_scan_agg_body(const b2_scan_t& s, const LD& ld, const b2_aggs_arg& aggs,
                                                  int64_t (*sh_acc)[B2_BLOCK], int32_t (*sh_cnt)[B2_BLOCK], int tid) {
   bool full;
@@ -79,7 +88,15 @@ __device__ __forceinline__ void b2_scan_agg_body(const b2_scan_t& s, const LD& l
     if (c.valid || c.dtype == B2_F64) ok &= ~b2_null_bits<R>(c, ld.row0, bits, raw);
     sh_cnt[a][tid] += __popc(ok);
     int64_t acc = sh_acc[a][tid];
-    switch (b2_agg_kind(ag.op, c.dtype)) {
+    const int kind = b2_agg_kind<BITS>(ag.op, c.dtype);
+    if (BITS && kind >= B2_K_AND) {
+      if (kind == B2_K_AND) acc = b2_fold_batch<R, B2_K_AND>(acc, raw, ok);
+      else if (kind == B2_K_OR) acc = b2_fold_batch<R, B2_K_OR>(acc, raw, ok);
+      else acc = b2_fold_batch<R, B2_K_XOR>(acc, raw, ok);
+      sh_acc[a][tid] = acc;
+      continue;
+    }
+    switch (kind) {
       case B2_K_SUM_I: acc = b2_fold_batch<R, B2_K_SUM_I>(acc, raw, ok); break;
       case B2_K_SUM_F: acc = b2_fold_batch<R, B2_K_SUM_F>(acc, raw, ok); break;
       case B2_K_SUMF_I: acc = b2_fold_batch<R, B2_K_SUMF_I>(acc, raw, ok); break;
@@ -93,7 +110,7 @@ __device__ __forceinline__ void b2_scan_agg_body(const b2_scan_t& s, const LD& l
   }
 }
 
-template <bool PIPE>
+template <bool PIPE, bool BITS>
 __global__ void __launch_bounds__(PIPE ? B2_PIPE_THREADS : B2_BLOCK)
 b2_scan_agg_kernel(const __grid_constant__ b2_scan_t s, const __grid_constant__ b2_pipe_t pp,
                    const __grid_constant__ b2_aggs_arg aggs, b2_partial* __restrict__ partials) {
@@ -102,12 +119,12 @@ b2_scan_agg_kernel(const __grid_constant__ b2_scan_t s, const __grid_constant__ 
   const int tid = threadIdx.x;
   if (tid < B2_BLOCK) {
     for (int a = 0; a < aggs.n; ++a) {
-      sh_acc[a][tid] = b2_identity(aggs.a[a].op);
+      sh_acc[a][tid] = b2_identity<BITS>(aggs.a[a].op);
       sh_cnt[a][tid] = 0;
     }
   }
-  if (PIPE) b2_tile_pipeline(s, pp, [&](const auto& ld) { b2_scan_agg_body<B2_PIPE_R>(s, ld, aggs, sh_acc, sh_cnt, tid); });
-  else b2_tile_direct<B2_AGG_R>(s, [&](const auto& ld) { b2_scan_agg_body<B2_AGG_R>(s, ld, aggs, sh_acc, sh_cnt, tid); });
+  if (PIPE) b2_tile_pipeline(s, pp, [&](const auto& ld) { b2_scan_agg_body<B2_PIPE_R, BITS>(s, ld, aggs, sh_acc, sh_cnt, tid); });
+  else b2_tile_direct<B2_AGG_R>(s, [&](const auto& ld) { b2_scan_agg_body<B2_AGG_R, BITS>(s, ld, aggs, sh_acc, sh_cnt, tid); });
   __syncthreads();
   // block reduction in a fixed order: thread a folds the 256 per-thread slots of aggregate a.
   // (int32 per-thread counts cannot overflow: a thread sees < 2^31 rows of a < 2^31-row partition)
@@ -115,9 +132,9 @@ b2_scan_agg_kernel(const __grid_constant__ b2_scan_t s, const __grid_constant__ 
     const int a = tid;
     const int op = aggs.a[a].op;
     const int dt = aggs.a[a].col >= 0 ? s.cols[aggs.a[a].col].dtype : B2_I64;
-    int64_t r = b2_identity(op), c = 0;
+    int64_t r = b2_identity<BITS>(op), c = 0;
     for (int t = 0; t < B2_BLOCK; ++t) {
-      r = b2_combine(op, dt, r, sh_acc[a][t]);
+      r = b2_combine<BITS>(op, dt, r, sh_acc[a][t]);
       c += sh_cnt[a][t];
     }
     partials[blockIdx.x].acc[a] = r;
@@ -376,7 +393,9 @@ static int32_t b2_check_aggs(const b2_scan_t* s, const b2_agg_t* aggs, int32_t n
   out->n = naggs;
   for (int a = 0; a < naggs; ++a) {
     B2_REQUIRE(aggs[a].col >= -1 && aggs[a].col < s->ncols, "agg column out of range");
-    B2_REQUIRE(aggs[a].op >= B2_AGG_SUM && aggs[a].op <= B2_AGG_COUNT, "bad agg op");
+    B2_REQUIRE(aggs[a].op >= B2_AGG_SUM && aggs[a].op <= B2_AGG_XOR, "bad agg op");
+    B2_REQUIRE(aggs[a].op < B2_AGG_AND || aggs[a].col < 0 || s->cols[aggs[a].col].dtype != B2_F64,
+               "bitwise aggregates take int64 or boolean inputs");
     out->a[a] = aggs[a];
   }
   return B2_OK;
@@ -394,16 +413,20 @@ int32_t b2_scan_agg(const b2_scan_t* scan, const b2_agg_t* aggs, int32_t naggs, 
   b2_pipe_t pp;
   b2_make_pipe(*scan, &pp);
   b2_partial* partials = reinterpret_cast<b2_partial*>(ws);
+  bool bits = false;
+  for (int a = 0; a < naggs; ++a) bits |= aa.a[a].op >= B2_AGG_AND;
   int grid;
   if (pp.enabled) {
-    grid = b2_pipe_grid(b2_scan_agg_kernel<true>, pp, scan->n);
+    auto k = bits ? b2_scan_agg_kernel<true, true> : b2_scan_agg_kernel<true, false>;
+    grid = b2_pipe_grid(k, pp, scan->n);
     if (grid > B2_MAX_PARTIALS) grid = B2_MAX_PARTIALS;
-    b2_scan_agg_kernel<true><<<grid, B2_PIPE_THREADS, pp.smem_bytes, st>>>(*scan, pp, aa, partials);
+    k<<<grid, B2_PIPE_THREADS, pp.smem_bytes, st>>>(*scan, pp, aa, partials);
   } else {
+    auto k = bits ? b2_scan_agg_kernel<false, true> : b2_scan_agg_kernel<false, false>;
     int64_t nblk = (scan->n + B2_AGG_ROWS_PER_BLOCK - 1) / B2_AGG_ROWS_PER_BLOCK;
-    grid = b2_wave_grid(b2_scan_agg_kernel<false>, B2_BLOCK, nblk);
+    grid = b2_wave_grid(k, B2_BLOCK, nblk);
     if (grid > B2_MAX_PARTIALS) grid = B2_MAX_PARTIALS;
-    b2_scan_agg_kernel<false><<<grid, B2_BLOCK, 0, st>>>(*scan, pp, aa, partials);
+    k<<<grid, B2_BLOCK, 0, st>>>(*scan, pp, aa, partials);
   }
   B2_CHECK_LAUNCH("b2_scan_agg_kernel");
   if (naggs > 0) {

@@ -536,9 +536,9 @@ int32_t b2_groupby_dense_hot(const b2_scan_t* scan, int32_t key_col, int64_t kmi
   B2_REQUIRE(nslots >= 2 && nslots < ((int64_t)1 << 31), "nslots must cover the key range plus the NULL slot, below 2^31");
   if (scan->n == 0) return B2_OK;
   b2_hot_t hot;
-  b2_make_hot(*scan, aa, *st, &hot);
+  b2_make_hot(*scan, aa, *st, &hot, true);
   const int cap = b2_hh_capacity(hot.narrays);
-  if (cap == 0)   // nothing SUM-like to privatise (MIN / MAX only): the plain kernel
+  if (cap == 0)   // nothing SUM-like or bitwise to privatise (MIN / MAX only): the plain kernel
     return b2_groupby_dense(scan, key_col, kmin, nslots, aggs, naggs, st, stream);
   const size_t smem = b2_hh_smem_bytes(hot.narrays);
   if (smem > 48 * 1024)

@@ -159,6 +159,9 @@ __device__ __forceinline__ void b2_join_agg_body(const b2_scan_t& s, const b2_gl
       case B2_K_MAX_I: acc = b2_fold_batch<R, B2_K_MAX_I>(acc, x, ok); break;
       case B2_K_MIN_F: acc = b2_fold_batch<R, B2_K_MIN_F>(acc, x, ok); break;
       case B2_K_MAX_F: acc = b2_fold_batch<R, B2_K_MAX_F>(acc, x, ok); break;
+      case B2_K_AND: acc = b2_fold_batch<R, B2_K_AND>(acc, x, ok); break;
+      case B2_K_OR: acc = b2_fold_batch<R, B2_K_OR>(acc, x, ok); break;
+      case B2_K_XOR: acc = b2_fold_batch<R, B2_K_XOR>(acc, x, ok); break;
       default: break;
     }
     sh_acc[a][tid] = acc;
@@ -339,7 +342,7 @@ int32_t b2_join_agg(const b2_scan_t* scan, int32_t probe_key, const b2_jointable
   for (int a = 0; a < naggs; ++a) {
     const b2_joinagg_t& ag = aggs[a];
     B2_REQUIRE(ag.combine >= B2_JA_P && ag.combine <= B2_JA_ROWS, "bad combine");
-    B2_REQUIRE(ag.op >= B2_AGG_SUM && ag.op <= B2_AGG_COUNT, "bad agg op");
+    B2_REQUIRE(ag.op >= B2_AGG_SUM && ag.op <= B2_AGG_XOR, "bad agg op");
     const bool needp = ag.combine != B2_JA_B && ag.combine != B2_JA_ROWS;
     const bool needb = ag.combine != B2_JA_P && ag.combine != B2_JA_ROWS;
     B2_REQUIRE(!needp || (ag.pcol >= 0 && ag.pcol < scan->ncols), "probe column out of range");
@@ -350,6 +353,7 @@ int32_t b2_join_agg(const b2_scan_t* scan, int32_t probe_key, const b2_jointable
     if (!needp) ja.a[a].pcol = -1;
     if (!needb) ja.a[a].bcol = -1;
     const bool isf = (needp && scan->cols[ag.pcol].dtype == B2_F64) || (needb && build_cols[ag.bcol].dtype == B2_F64);
+    B2_REQUIRE(ag.combine == B2_JA_ROWS || ag.op < B2_AGG_AND || !isf, "bitwise aggregates take int64 inputs");
     fa.op[a] = ag.combine == B2_JA_ROWS ? B2_AGG_COUNT : ag.op;
     fa.dtype[a] = isf ? B2_F64 : B2_I64;
     if (ag.combine == B2_JA_ROWS) ja.a[a].op = B2_AGG_COUNT;

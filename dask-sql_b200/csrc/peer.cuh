@@ -59,6 +59,9 @@ __device__ __forceinline__ int64_t b2_peer_combine(int op, int64_t a, int64_t b)
     case B2_PEER_SUM_F64: return __double_as_longlong(__longlong_as_double(a) + __longlong_as_double(b));
     case B2_PEER_SUM_I64: return (int64_t)((uint64_t)a + (uint64_t)b);      // wraps like numpy
     case B2_PEER_MIN_I64: return a < b ? a : b;
+    case B2_PEER_AND_I64: return a & b;
+    case B2_PEER_OR_I64: return a | b;
+    case B2_PEER_XOR_I64: return a ^ b;
     default: return a > b ? a : b;                                            // B2_PEER_MAX_I64
   }
 }
@@ -143,7 +146,7 @@ int32_t b2_peer_merge(const b2_peer_merge_t* m, void* stream) {
   for (int p = 0; p < m->world; ++p) B2_REQUIRE(m->peer_base[p], "null peer base");
   for (int a = 0; a < m->narrays; ++a) {
     B2_REQUIRE(m->out[a] && m->array_off[a] % 16 == 0, "null or misaligned array");
-    B2_REQUIRE(m->ops[a] >= B2_PEER_SUM_F64 && m->ops[a] <= B2_PEER_MAX_I64, "bad op");
+    B2_REQUIRE(m->ops[a] >= B2_PEER_SUM_F64 && m->ops[a] <= B2_PEER_XOR_I64, "bad op");
   }
   // enough CTAs to keep world x narrays 16-byte requests per thread in flight on every SM, few enough that
   // a concurrent NCCL kernel (the next step's lookup broadcast) always finds room beside the spinning grid

@@ -141,21 +141,24 @@ b2_iota_kernel(int32_t* __restrict__ out, int64_t n) {
 }
 
 __global__ void __launch_bounds__(B2_BLOCK)
-b2_bitmap_or_kernel(uint32_t* __restrict__ dst, const uint32_t* __restrict__ src, int64_t nwords) {
-  for (int64_t i = (int64_t)blockIdx.x * B2_BLOCK + threadIdx.x; i < nwords; i += (int64_t)gridDim.x * B2_BLOCK)
-    dst[i] |= src[i];
+b2_bitwise_combine_kernel(uint32_t* __restrict__ dst, const uint32_t* __restrict__ src, int64_t nwords, int op) {
+  for (int64_t i = (int64_t)blockIdx.x * B2_BLOCK + threadIdx.x; i < nwords; i += (int64_t)gridDim.x * B2_BLOCK) {
+    const uint32_t a = dst[i], b = src[i];
+    dst[i] = op == B2_AGG_AND ? a & b : op == B2_AGG_OR ? a | b : a ^ b;
+  }
 }
 
 extern "C" {
 
-// dst |= src over nwords 32-bit words: merges the presence bitmaps of per-GPU dense group tables
+// dst = dst <op> src over nwords 32-bit words: the fold of bitwise accumulators exchanged between GPUs
 // (NCCL offers no bitwise reduction).
-int32_t b2_bitmap_or(uint32_t* dst, const uint32_t* src, int64_t nwords, void* stream) {
+int32_t b2_bitwise_combine(uint32_t* dst, const uint32_t* src, int64_t nwords, int32_t op, void* stream) {
   B2_REQUIRE((dst && src) || nwords == 0, "null argument");
+  B2_REQUIRE(op == B2_AGG_AND || op == B2_AGG_OR || op == B2_AGG_XOR, "bad bitwise op");
   if (nwords <= 0) return B2_OK;
-  int grid = b2_wave_grid(b2_bitmap_or_kernel, B2_BLOCK, (nwords + B2_BLOCK - 1) / B2_BLOCK);
-  b2_bitmap_or_kernel<<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(dst, src, nwords);
-  B2_CHECK_LAUNCH("b2_bitmap_or_kernel");
+  int grid = b2_wave_grid(b2_bitwise_combine_kernel, B2_BLOCK, (nwords + B2_BLOCK - 1) / B2_BLOCK);
+  b2_bitwise_combine_kernel<<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(dst, src, nwords, op);
+  B2_CHECK_LAUNCH("b2_bitwise_combine_kernel");
   return B2_OK;
 }
 

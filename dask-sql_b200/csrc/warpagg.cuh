@@ -25,14 +25,17 @@ struct b2_hot_t {                   // lives in kernel-parameter space; smem poi
   int8_t cnt_arr[B2_MAX_AGGS];
   int8_t rows_arr;
   int8_t is_f64[B2_HOT_MAX_ARRAYS]; // array holds doubles (else int64)
+  int8_t bit_op[B2_HOT_MAX_ARRAYS]; // B2_AGG_AND / OR / XOR: a bitwise accumulator (heavy-hitter path only); 0 = a sum
 };
 
 static inline size_t b2_hot_smem_bytes(const b2_hot_t& h) {
   return h.enabled ? (size_t)B2_HOT_SLOTS * 4 + (size_t)h.narrays * B2_WARPS * B2_HOT_SLOTS * 8 : 0;
 }
 
-// host: which accumulator arrays the table carries (SUM-like ones and counts)
-static inline void b2_make_hot(const b2_scan_t& s, const b2_aggs_arg& aa, const b2_aggstate_t& st, b2_hot_t* h) {
+// host: which accumulator arrays the table carries (SUM-like ones and counts; with `bitwise`, which only the
+// heavy-hitter kernel sets, also AND / OR / XOR accumulators)
+static inline void b2_make_hot(const b2_scan_t& s, const b2_aggs_arg& aa, const b2_aggstate_t& st, b2_hot_t* h,
+                               bool bitwise = false) {
   memset(h, 0, sizeof(*h));
   h->rows_arr = -1;
   int n = 0;
@@ -45,6 +48,10 @@ static inline void b2_make_hot(const b2_scan_t& s, const b2_aggs_arg& aa, const 
     if (st.acc[a] && (op == B2_AGG_SUM || op == B2_AGG_SUMF)) {
       if (n >= B2_HOT_MAX_ARRAYS) { fits = false; break; }
       h->is_f64[n] = (op == B2_AGG_SUMF || dt == B2_F64) ? 1 : 0;
+      h->acc_arr[a] = (int8_t)n++;
+    } else if (st.acc[a] && bitwise && op >= B2_AGG_AND && op <= B2_AGG_XOR) {
+      if (n >= B2_HOT_MAX_ARRAYS) { fits = false; break; }
+      h->bit_op[n] = (int8_t)op;
       h->acc_arr[a] = (int8_t)n++;
     }
     if (st.cnt[a]) {
@@ -96,17 +103,30 @@ __device__ __forceinline__ int64_t b2_group_sum(uint32_t m, int64_t v, int maxc,
   }
   return acc;
 }
-template <bool IS_MIN>
-__device__ __forceinline__ int64_t b2_group_minmax(uint32_t m, int64_t v, int maxc, int lane) {
+// the same for an order-free op: KIND = B2_K_MIN_I / MAX_I (ints or ordered images) / AND / OR / XOR
+template <int KIND>
+__device__ __forceinline__ int64_t b2_group_reduce(uint32_t m, int64_t v, int maxc, int lane) {
   uint32_t others = m & ~(1u << lane);
   int64_t acc = v;
   for (int it = 1; it < maxc; ++it) {
     const int src = others ? __ffs(others) - 1 : lane;
     others &= others - 1;
     const int64_t o = __shfl_sync(FULL_MASK, v, src);
-    if (src != lane) acc = IS_MIN ? (o < acc ? o : acc) : (o > acc ? o : acc);
+    if (src != lane) {
+      if (KIND == B2_K_MIN_I) acc = o < acc ? o : acc;
+      else if (KIND == B2_K_MAX_I) acc = o > acc ? o : acc;
+      else if (KIND == B2_K_AND) acc &= o;
+      else if (KIND == B2_K_OR) acc |= o;
+      else acc ^= o;
+    }
   }
   return acc;
+}
+template <int KIND>
+__device__ __forceinline__ void b2_group_reduce_flush(void* acc, int64_t slot, uint32_t m, int64_t v, int maxc, int lane,
+                                                      bool issue) {
+  const int64_t t = b2_group_reduce<KIND>(m, v, maxc, lane);
+  if (issue) b2_atomic_k<KIND>(acc, slot, t);   // one REDG per group
 }
 
 // Does this batch repeat slots?  One MATCH on the first step's rows: warp-uniform answer.
@@ -235,14 +255,21 @@ __device__ __forceinline__ void b2_apply_aggs_grouped(const b2_scan_t& s, const 
           }
         }
       } else {
-        const bool is_min = kind == B2_K_MIN_I || kind == B2_K_MIN_F;
+        // MIN / MAX (float values as their ordered images) and the bitwise ops: lanes without a value
+        // contribute the op's identity
         const bool flt = kind == B2_K_MIN_F || kind == B2_K_MAX_F;
-        const int64_t ident = is_min ? LLONG_MAX : LLONG_MIN;
+        int64_t ident = 0;
+        if (kind == B2_K_MIN_I || kind == B2_K_MIN_F) ident = LLONG_MAX;
+        else if (kind == B2_K_MAX_I || kind == B2_K_MAX_F) ident = LLONG_MIN;
+        else if (kind == B2_K_AND) ident = -1;
         const int64_t v = mine ? (flt ? b2_ordered_from_bits(raw[j]) : raw[j]) : ident;
-        const int64_t t = is_min ? b2_group_minmax<true>(grp[j], v, mc, lane) : b2_group_minmax<false>(grp[j], v, mc, lane);
-        if (leader && any) {
-          if (is_min) atomicMin(reinterpret_cast<long long*>(acc) + slot[j], (long long)t);
-          else atomicMax(reinterpret_cast<long long*>(acc) + slot[j], (long long)t);
+        const bool issue = leader && any;
+        switch (kind) {
+          case B2_K_MIN_I: case B2_K_MIN_F: b2_group_reduce_flush<B2_K_MIN_I>(acc, slot[j], grp[j], v, mc, lane, issue); break;
+          case B2_K_MAX_I: case B2_K_MAX_F: b2_group_reduce_flush<B2_K_MAX_I>(acc, slot[j], grp[j], v, mc, lane, issue); break;
+          case B2_K_AND: b2_group_reduce_flush<B2_K_AND>(acc, slot[j], grp[j], v, mc, lane, issue); break;
+          case B2_K_OR: b2_group_reduce_flush<B2_K_OR>(acc, slot[j], grp[j], v, mc, lane, issue); break;
+          default: b2_group_reduce_flush<B2_K_XOR>(acc, slot[j], grp[j], v, mc, lane, issue); break;
         }
       }
       if (hot.enabled) __syncwarp();   // shared-table updates of this step before the next step's
@@ -384,8 +411,11 @@ __device__ __forceinline__ b2_hh_smem b2_hh_init(const b2_hot_t& hot, const int3
   // float partials start at -0.0 (the INT64_MIN bit pattern) and only ever receive x + 0.0: a partial that
   // still reads -0.0 saw no row, -0.0 + -0.0 = -0.0 survives the fold, and anything else (+0.0 included)
   // means "this CTA met the hitter" -- the same convention as the global accumulators' existence mark
-  for (int i = threadIdx.x; i < hot.narrays * cap * B2_BLOCK; i += blockDim.x)
-    hs.part[i] = hot.is_f64[i / (cap * B2_BLOCK)] ? (int64_t)0x8000000000000000LL : 0;
+  // bitwise partials start at the op's identity (all ones for AND)
+  for (int i = threadIdx.x; i < hot.narrays * cap * B2_BLOCK; i += blockDim.x) {
+    const int k = i / (cap * B2_BLOCK);
+    hs.part[i] = hot.is_f64[k] ? (int64_t)0x8000000000000000LL : hot.bit_op[k] == B2_AGG_AND ? -1 : 0;
+  }
   __syncthreads();
   if (threadIdx.x == 0) {
     // most frequent first; a hitter whose bucket is taken is simply not tracked (its rows take atomics)
@@ -428,6 +458,11 @@ __device__ __forceinline__ void b2_hh_batch(void* acc, int64_t* cnt, const int64
       else if (KIND == B2_K_SUM_F)
         *p = __double_as_longlong(__longlong_as_double(*p) + __dadd_rn(__longlong_as_double(raw[j]), 0.0));
       else *p = __double_as_longlong(__longlong_as_double(*p) + __dadd_rn((double)raw[j], 0.0));
+    } else if (h >= 0 && part_acc && (KIND == B2_K_AND || KIND == B2_K_OR || KIND == B2_K_XOR)) {
+      int64_t* p = part_acc + h * stride;
+      if (KIND == B2_K_AND) *p &= raw[j];
+      else if (KIND == B2_K_OR) *p |= raw[j];
+      else *p ^= raw[j];
     } else {
       b2_atomic_k<KIND>(acc, slot[j], raw[j]);
     }
@@ -491,14 +526,17 @@ __device__ __forceinline__ void b2_apply_aggs_hh(const b2_scan_t& s, const LD& l
       case B2_K_MAX_I: b2_hh_batch<R, B2_K_MAX_I>(acc, cnt, slot, raw, ok, hit, pa, pc, stride); break;
       case B2_K_MIN_F: b2_hh_batch<R, B2_K_MIN_F>(acc, cnt, slot, raw, ok, hit, pa, pc, stride); break;
       case B2_K_MAX_F: b2_hh_batch<R, B2_K_MAX_F>(acc, cnt, slot, raw, ok, hit, pa, pc, stride); break;
+      case B2_K_AND: b2_hh_batch<R, B2_K_AND>(acc, cnt, slot, raw, ok, hit, pa, pc, stride); break;
+      case B2_K_OR: b2_hh_batch<R, B2_K_OR>(acc, cnt, slot, raw, ok, hit, pa, pc, stride); break;
+      case B2_K_XOR: b2_hh_batch<R, B2_K_XOR>(acc, cnt, slot, raw, ok, hit, pa, pc, stride); break;
       default: b2_hh_batch<R, B2_K_NONE>(acc, cnt, slot, raw, ok, hit, pa, pc, stride); break;
     }
   }
 }
 
 // CTA epilogue: fold the 256 thread partials of every (array, hitter) and issue one global atomic each.
-// A hitter that this CTA never met contributes exact zeros, which are skipped (an untouched float SUM
-// accumulator must keep its -0.0 "no group" mark).
+// A hitter that this CTA never met contributes exact zeros (or, for AND, all ones), which are skipped (an
+// untouched float SUM accumulator must keep its -0.0 "no group" mark).
 __device__ __forceinline__ void b2_hh_flush(const b2_hot_t& hot, const b2_hh_smem& hs, const int32_t* __restrict__ d_hot,
                                             const b2_aggs_arg& aggs, const b2_aggstate_t& st) {
   __syncthreads();
@@ -509,6 +547,28 @@ __device__ __forceinline__ void b2_hh_flush(const b2_hot_t& hot, const b2_hh_sme
     if (slot < 0) continue;
     const int64_t* p = hs.part + (size_t)k * B2_BLOCK;
     const bool f = hot.is_f64[arr];
+    const int bop = hot.bit_op[arr];
+    if (bop) {
+      uint64_t b = bop == B2_AGG_AND ? ~0ULL : 0ULL;
+      for (int t = lane; t < B2_BLOCK; t += 32) {
+        const uint64_t v = (uint64_t)p[t];
+        b = bop == B2_AGG_AND ? b & v : bop == B2_AGG_OR ? b | v : b ^ v;
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        const uint64_t v = __shfl_xor_sync(FULL_MASK, b, o);
+        b = bop == B2_AGG_AND ? b & v : bop == B2_AGG_OR ? b | v : b ^ v;
+      }
+      if (lane != 0 || b == (bop == B2_AGG_AND ? ~0ULL : 0ULL)) continue;   // the identity changes nothing
+      for (int a = 0; a < aggs.n; ++a) {
+        if (hot.acc_arr[a] != arr) continue;
+        unsigned long long* d = reinterpret_cast<unsigned long long*>(st.acc[a]) + slot;
+        if (bop == B2_AGG_AND) atomicAnd(d, b);
+        else if (bop == B2_AGG_OR) atomicOr(d, b);
+        else atomicXor(d, b);
+      }
+      continue;
+    }
     double fs = -0.0;
     uint64_t is = 0;
     for (int t = lane; t < B2_BLOCK; t += 32) {

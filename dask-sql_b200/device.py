@@ -427,14 +427,10 @@ class GroupTable:
         for a, ((col, op), dt) in enumerate(zip(self.specs, agg_dtypes)):
             acc = cnt = None
             if col >= 0 and op != L.AGG_COUNT:
-                if op == L.AGG_MIN:
-                    acc = new(alloc, torch.int64, (1 << 63) - 1)
-                elif op == L.AGG_MAX:
-                    acc = new(alloc, torch.int64, -(1 << 63))
-                elif op == L.AGG_SUMF or dt == F64:
+                if op == L.AGG_SUMF or (op == L.AGG_SUM and dt == F64):
                     acc = new(alloc, torch.float64, -0.0 if a == indicator else 0.0)
                 else:
-                    acc = new(alloc, torch.int64, 0)
+                    acc = new(alloc, torch.int64, L.agg_identity(op))
             if col >= 0 and (op == L.AGG_COUNT or need_cnt[a]):
                 cnt = new(alloc, torch.int64, 0)
             self.acc.append(acc)

@@ -643,7 +643,10 @@ def execute(frame: LazyFrame, needed: Optional[Sequence[str]] = None, top: bool 
 # ---------------------------------------------------------------------------------------------
 # aggregation
 # ---------------------------------------------------------------------------------------------
-MOMENT_FUNCS = ("var_samp", "var_pop", "stddev_samp", "stddev_pop")
+MOMENT_FUNCS = ("var_samp", "var_pop", "stddev_samp", "stddev_pop", "regr_sxx", "regr_syy")
+# bitwise aggregates -> kernel op; EVERY is the AND of the 0/1 boolean input
+BIT_FUNCS = {"bit_and": L.AGG_AND, "bit_or": L.AGG_OR, "bit_xor": L.AGG_XOR, "every": L.AGG_AND}
+_BIT_REDUCE = {L.AGG_AND: "and", L.AGG_OR: "or", L.AGG_XOR: "xor"}
 
 
 class KAgg:
@@ -705,6 +708,14 @@ class AggPlan:
             elif fn in ("min", "max"):
                 a = self._slot(e, L.AGG_MIN if fn == "min" else L.AGG_MAX, nul)
                 self.outs.append((out, fn, a, self._cnt(e) if nul else None, e.dtype, lg))
+            elif fn in BIT_FUNCS:
+                if e.dtype == F64:
+                    raise TypeError(f"{fn.upper()} takes an integer or boolean input, not a float")
+                a = self._slot(e, BIT_FUNCS[fn], nul)
+                # a group without a non-NULL input is NULL: a numpy int64 result would turn into float64 on
+                # the way to pandas and lose the low bits of large values, so it becomes nullable Int64
+                self.outs.append((out, fn, a, self._cnt(e) if nul else None, e.dtype,
+                                  "Int64" if nul and lg == "int64" else lg))
             else:
                 raise NotImplementedError(f"aggregate function {fn} is a 'next' row of the hot-path scope")
         if len(self.kaggs) > L.MAX_AGGS:
@@ -862,8 +873,7 @@ def global_aggregate(parts: List[Part], pred, plan: AggPlan, sharded: bool) -> P
         ga.update(ctx.scan())
         _kernel_event_end(ev)
     if ga is None:
-        acc = np.array([{L.AGG_MIN: (1 << 63) - 1, L.AGG_MAX: -(1 << 63)}.get(ka.op, 0) for ka in plan.kaggs] + [0],
-                       dtype=np.int64)
+        acc = np.array([L.agg_identity(ka.op) for ka in plan.kaggs] + [0], dtype=np.int64)
         cnt = np.zeros(k + 1, dtype=np.int64)
     else:
         acc, cnt = ga.result()
@@ -887,16 +897,20 @@ def _finish_global(plan: AggPlan, acc, cnt, dev, float_acc=None) -> Part:
             val, dt, lgo = n_valid, I64, "int64"
         elif fn in MOMENT_FUNCS:
             dt, lgo = F64, "float64"
-            ddof = 0 if fn.endswith("pop") else 1
+            ddof = 0 if fn.endswith("pop") or fn.startswith("regr") else 1
             if n_valid <= ddof:
                 val = None
             else:
                 s1 = acc[a:a + 1].view(np.float64)[0].item()
                 a2 = plan.second[name]
                 s2 = acc[a2:a2 + 1].view(np.float64)[0].item()
-                val = max((s2 - s1 * s1 / n_valid) / (n_valid - ddof), 0.0)
+                # REGR_SXX / REGR_SYY are the sum of squared deviations itself, not divided by n
+                val = max((s2 - s1 * s1 / n_valid) / (1 if fn.startswith("regr") else n_valid - ddof), 0.0)
                 if fn.startswith("stddev"):
                     val = val ** 0.5
+        elif fn in BIT_FUNCS:
+            dt, lgo = (U8, "bool") if fn == "every" else (I64, lg)
+            val = None if n_valid == 0 else (bool(acc[a]) if fn == "every" else int(acc[a]))
         elif fn == "sum":
             dt, lgo = (F64, lg if in_dt == F64 else "float64") if is_f else (I64, lg if lg != "bool" else "int64")
             val = None if n_valid == 0 else (acc[a:a + 1].view(np.float64)[0].item() if is_f else int(acc[a]))
@@ -940,6 +954,8 @@ def _allreduce_global(acc, cnt, plan: AggPlan, dev):
             out[i] = col.min()
         elif ka.op == L.AGG_MAX:
             out[i] = col.max()
+        elif ka.op in _BIT_REDUCE:
+            out[i] = getattr(np, f"bitwise_{_BIT_REDUCE[ka.op]}").reduce(col)
     return out, cnts.sum(axis=0)
 
 
@@ -1006,7 +1022,10 @@ def grouped_aggregate(parts, pred, gexprs, gnames, plan: AggPlan, child, sharded
         for g, e, lg in zip(gnames, gexprs, glog):
             out[g] = DeviceColumn(torch.empty(0, dtype=_TORCH_DT[e.dtype], device=dev), None, e.dtype, lg)
         for name, fn, a, c, in_dt, lg in plan.outs:
-            dt = I64 if fn in ("size", "count") else (F64 if fn == "mean" or in_dt == F64 else I64)
+            if fn == "every":
+                dt = U8
+            else:
+                dt = I64 if fn in ("size", "count") else (F64 if fn in ("mean",) + MOMENT_FUNCS or in_dt == F64 else I64)
             out[name] = DeviceColumn(torch.empty(0, dtype=_TORCH_DT[dt], device=dev), None, dt)
         return out
 
@@ -1295,7 +1314,7 @@ def _merge_dense(t: D.GroupTable, plan: AggPlan, sharded: bool, dev, keep=None) 
         accs, cnts = [], []
         for i, (ka, acc, cnt) in enumerate(zip(plan.kaggs, t.acc, t.cnt)):
             accs.append(None if acc is None else
-                        P.reduce_scatter_(acc, {L.AGG_MIN: "min", L.AGG_MAX: "max"}.get(ka.op, "sum"),
+                        P.reduce_scatter_(acc, {L.AGG_MIN: "min", L.AGG_MAX: "max", **_BIT_REDUCE}.get(ka.op, "sum"),
                                           out=kept(("a", i), acc)))
             cnts.append(None if cnt is None else P.reduce_scatter_(cnt, "sum", out=kept(("c", i), cnt)))
         rows = None if t.rows is None else P.reduce_scatter_(t.rows, "sum", out=kept("r", t.rows))
@@ -1331,11 +1350,12 @@ def _finish_outputs(plan: AggPlan, acc_cols, cnt_cols, rows_col, n, out: Part):
         env["a"] = acc
         if fn in MOMENT_FUNCS:
             env["b"] = acc_cols[plan.second[name]]
-            ddof = 0 if fn.endswith("pop") else 1
+            ddof = 0 if fn.endswith("pop") or fn.startswith("regr") else 1
             nf = E.cast(ColRef("c", I64), F64)
             s1, s2 = ColRef("a", F64), ColRef("b", F64)
-            var = E.binop("truediv", E.binop("sub", s2, E.binop("truediv", E.binop("mul", s1, s1), nf)),
-                          E.binop("sub", nf, float(ddof)))
+            var = E.binop("sub", s2, E.binop("truediv", E.binop("mul", s1, s1), nf))
+            if not fn.startswith("regr"):          # REGR_SXX / REGR_SYY: the sum of squared deviations itself
+                var = E.binop("truediv", var, E.binop("sub", nf, float(ddof)))
             var = E.case(E.binop("lt", var, 0.0), Lit(0.0), var)      # a constant group may round to -1e-17
             val = E.unop("sqrt", var) if fn.startswith("stddev") else var
             col = eval_expr(env, E.case(E.binop("gt", ColRef("c", I64), ddof), val, Lit(None, F64)))
@@ -1347,6 +1367,15 @@ def _finish_outputs(plan: AggPlan, acc_cols, cnt_cols, rows_col, n, out: Part):
             e = E.case(E.binop("gt", ColRef("c", I64), 0), e, Lit(None, F64))
             col = eval_expr(env, e)
             col.logical = "float64"
+        elif fn in BIT_FUNCS:
+            # a group without a non-NULL input still holds the op's identity: NULL it by the count
+            val = ColRef("a", I64)
+            if fn == "every":
+                val = E.binop("ne", val, 0)
+            if cnt is not None:
+                val = E.case(E.binop("gt", ColRef("c", I64), 0), val, Lit(None, val.dtype))
+            col = eval_expr(env, val) if not isinstance(val, ColRef) else acc
+            col = DeviceColumn(col.data, col.valid, val.dtype, "bool" if fn == "every" else lg)
         else:
             is_f = (in_dt == F64)
             val: Expr = ColRef("a", I64 if (fn in ("min", "max") or not is_f) else F64)
@@ -1757,7 +1786,8 @@ class PreparedStar:
             arrays, accs, cnts, rows = [], [], [], None      # arrays: (tensor, op) in the kernel's order
             for ka, acc, cnt in zip(self.plan.kaggs, t.acc, t.cnt):
                 if acc is not None:
-                    op = {L.AGG_MIN: L.PEER_MIN_I64, L.AGG_MAX: L.PEER_MAX_I64}.get(
+                    op = {L.AGG_MIN: L.PEER_MIN_I64, L.AGG_MAX: L.PEER_MAX_I64, L.AGG_AND: L.PEER_AND_I64,
+                          L.AGG_OR: L.PEER_OR_I64, L.AGG_XOR: L.PEER_XOR_I64}.get(
                         ka.op, L.PEER_SUM_F64 if acc.dtype == torch.float64 else L.PEER_SUM_I64)
                     arrays.append((acc, op))
                 if cnt is not None:
@@ -2319,8 +2349,7 @@ def try_join_agg(src: AggSource, child: LazyFrame, aggs, pred, sharded) -> Optio
         _kernel_event_end(ev)
         first = False
     if first:
-        acc = np.array([{L.AGG_MIN: (1 << 63) - 1, L.AGG_MAX: -(1 << 63)}.get(ka.op, 0) for ka in plan.kaggs] + [0],
-                       dtype=np.int64)
+        acc = np.array([L.agg_identity(ka.op) for ka in plan.kaggs] + [0], dtype=np.int64)
         cnt = np.zeros(k + 1, dtype=np.int64)
     else:
         acc, cnt = acc_d.cpu().numpy(), cnt_d.cpu().numpy()

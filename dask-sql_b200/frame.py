@@ -59,12 +59,13 @@ class JoinSource(Source):
                 self.schema[n] = right.col_type(n)
 
 
-MOMENT_FUNCS = ("var_samp", "var_pop", "stddev_samp", "stddev_pop")
+MOMENT_FUNCS = ("var_samp", "var_pop", "stddev_samp", "stddev_pop", "regr_sxx", "regr_syy")
 
 
 class AggSource(Source):
     """group_cols: child columns; aggs: [(input child column or None, output name, fn)] with
-    fn in sum | count | mean | min | max | size | var_samp | var_pop | stddev_samp | stddev_pop."""
+    fn in sum | count | mean | min | max | size | var_samp | var_pop | stddev_samp | stddev_pop | regr_sxx |
+    regr_syy | bit_and | bit_or | bit_xor | every."""
 
     def __init__(self, child: "LazyFrame", group_cols, aggs, options=None):
         self.child, self.group_cols, self.aggs = child, list(group_cols), list(aggs)
@@ -77,6 +78,8 @@ class AggSource(Source):
                 self.schema[out] = (I64, "int64")
             elif fn == "mean" or fn in MOMENT_FUNCS:
                 self.schema[out] = (F64, "float64")
+            elif fn == "every":
+                self.schema[out] = (U8, "bool")
             else:
                 dt, lg = child.col_type(in_col)
                 if dt == U8:

@@ -125,7 +125,7 @@ def part_to_raw(part, raw_like):
 
 def merge_partials(parts: List, plan, nkeys: int):
     """Re-aggregate concatenated partial tables on this GPU with the same group-by kernels:
-    SUM of partial sums / counts / rows, MIN of mins, MAX of maxes."""
+    SUM of partial sums / counts / rows, MIN of mins, MAX of maxes, AND / OR / XOR of bitwise partials."""
     from .executor import Part, concat_parts
     from .frame import LazyFrame, TableSource, AggSource
     from .table import DeviceTable
@@ -141,7 +141,8 @@ def merge_partials(parts: List, plan, nkeys: int):
         fn = "sum"
         if n.startswith("a"):
             op = plan.kaggs[int(n[1:])].op
-            fn = {L.AGG_MIN: "min", L.AGG_MAX: "max"}.get(op, "sum")
+            fn = {L.AGG_MIN: "min", L.AGG_MAX: "max", L.AGG_AND: "bit_and", L.AGG_OR: "bit_or",
+                  L.AGG_XOR: "bit_xor"}.get(op, "sum")
         aggs.append((n, n, fn))
     keys = [f"k{i}" for i in range(nkeys)]
     merged = LazyFrame(AggSource(frame, keys, aggs))

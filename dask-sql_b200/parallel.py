@@ -79,7 +79,24 @@ def reduce_scatter_(t: torch.Tensor, op: str = "sum", out=None) -> torch.Tensor:
     n = t.numel()
     assert n % size == 0, "reduce_scatter_ needs a length that is a multiple of the world size"
     chunk = n // size
-    rop = {"sum": dist.ReduceOp.SUM, "min": dist.ReduceOp.MIN, "max": dist.ReduceOp.MAX}[op]
+    bitwise = op in ("and", "or", "xor")
+    rop = {"sum": dist.ReduceOp.SUM, "min": dist.ReduceOp.MIN, "max": dist.ReduceOp.MAX, "and": dist.ReduceOp.BAND,
+           "or": dist.ReduceOp.BOR, "xor": dist.ReduceOp.BXOR}[op]
+    if _backend() == "nccl" and bitwise:
+        # NCCL has no bitwise reduction: every rank receives the peers' copies of its slot chunk and folds
+        # them in rank order with b2_bitwise_combine (the op on 32-bit words is the op on 64-bit ones)
+        from . import _lib as L
+        from . import device as D
+        recv = torch.empty(n, dtype=t.dtype, device=t.device)
+        _timed(f"all_to_all[{t.dtype},{op}]", dist.all_to_all_single, recv, t.contiguous())
+        if out is None:
+            out = torch.empty(chunk, dtype=t.dtype, device=t.device)
+        out.copy_(recv[:chunk])
+        words = chunk * t.element_size() // 4
+        code = {"and": L.AGG_AND, "or": L.AGG_OR, "xor": L.AGG_XOR}[op]
+        for r in range(1, size):
+            L.bitwise_combine(out.data_ptr(), recv[r * chunk:(r + 1) * chunk].data_ptr(), words, code, D.stream_ptr())
+        return out
     if _backend() == "nccl":
         if out is None:
             out = torch.empty(chunk, dtype=t.dtype, device=t.device)

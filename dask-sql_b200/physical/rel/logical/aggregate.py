@@ -39,7 +39,12 @@ _EXECUTOR_NAME = {
     "stddev_pop": "stddev_pop", "stddevpop": "stddev_pop",
     "variance": "var_samp", "var_samp": "var_samp", "var": "var_samp",
     "var_pop": "var_pop", "variance_pop": "var_pop", "variancepop": "var_pop",
+    "bit_and": "bit_and", "bit_or": "bit_or", "bit_xor": "bit_xor", "every": "every",
+    "regr_count": "count", "regr_sxx": "regr_sxx", "regr_syy": "regr_syy",
 }
+# REGR_*(y, x): the one aggregate family with two inputs.  Only rows where BOTH are non-NULL count, so the
+# input is  x' = CASE WHEN y IS NOT NULL THEN x END  (y' likewise for REGR_SYY), and REGR_COUNT is COUNT(x').
+_REGR = {"regr_count": 1, "regr_sxx": 1, "regr_syy": 0}   # which argument is aggregated
 
 
 @dataclass
@@ -93,9 +98,16 @@ class DaskAggregatePlugin(BaseRelPlugin):
             if sql_name not in _EXECUTOR_NAME:
                 raise NotImplementedError(f"Aggregation function {sql_name} not implemented (yet).")
             args = node.getArgs(call)
-            if len(args) > 1:
+            if sql_name in _REGR:
+                vals = [value_of(a) for a in args]
+                if not all(isinstance(v, LazySeries) for v in vals):
+                    raise NotImplementedError(f"{sql_name.upper()} over a literal argument")
+                i = _REGR[sql_name]
+                arg = vals[i].where(vals[1 - i].notna())
+            elif len(args) > 1:
                 raise NotImplementedError("aggregates over more than one input column")
-            arg = value_of(args[0]) if args else None
+            else:
+                arg = value_of(args[0]) if args else None
             if arg is None and call.isDistinctAgg():
                 raise NotImplementedError("COUNT(DISTINCT *)")
             keep = call.getFilterExpr()

@@ -294,13 +294,22 @@ class Binder:
             if name in P.AGG_FUNCS:
                 name = "AVG" if name == "MEAN" else name
                 args = [] if e.star else [rec(a) for a in e.args]
-                if name != "COUNT" and len(args) != 1:
+                if name.startswith("REGR_"):
+                    if len(args) != 2:
+                        self.err(f"{name} takes exactly two arguments")
+                    if any(a.sql_type not in _NUMERIC + ("NULL",) for a in args):
+                        self.err(f"{name} takes numeric arguments")
+                elif name != "COUNT" and len(args) != 1:
                     self.err(f"{name} takes exactly one argument")
                 if any(a.contains_agg() for a in args):
                     self.err("Aggregate function calls cannot be nested")
-                if name == "COUNT":
+                if name.startswith("BIT_") and args[0].sql_type not in ("BIGINT", "INTEGER", "SMALLINT", "TINYINT"):
+                    self.err(f"{name} takes an integer argument, not {args[0].sql_type}")
+                if name == "EVERY" and args[0].sql_type != "BOOLEAN":
+                    self.err(f"{name} takes a BOOLEAN argument, not {args[0].sql_type}")
+                if name in ("COUNT", "REGR_COUNT"):
                     ty = "BIGINT"
-                elif name == "AVG" or name.startswith(("STDDEV", "VAR")):
+                elif name == "AVG" or name.startswith(("STDDEV", "VAR", "REGR_")):
                     ty = "DOUBLE"
                 elif name == "SUM":
                     ty = _norm_type(args[0].sql_type) if args[0].sql_type != "BOOLEAN" else "BIGINT"

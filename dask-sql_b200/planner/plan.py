@@ -92,7 +92,7 @@ for _n in ("Reference", "Call", "Literal", "Alias", "ScalarSubquery"):
 _ARROW = {"BIGINT": "Int64", "DOUBLE": "Float64", "BOOLEAN": "Boolean", "VARCHAR": "Utf8", "NULL": "Null",
           "INTEGER": "Int32", "FLOAT": "Float32"}
 AGG_FUNCS = {"SUM", "AVG", "COUNT", "MIN", "MAX", "MEAN", "STDDEV", "STDDEV_SAMP", "STDDEV_POP", "VAR_SAMP",
-             "VAR_POP", "VARIANCE"}
+             "VAR_POP", "VARIANCE", "BIT_AND", "BIT_OR", "BIT_XOR", "EVERY", "REGR_COUNT", "REGR_SXX", "REGR_SYY"}
 
 
 class PyExpr:

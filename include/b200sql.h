@@ -65,6 +65,9 @@ extern "C" {
 #define B2_AGG_MIN    2
 #define B2_AGG_MAX    3
 #define B2_AGG_COUNT  4   /* only the non-null count is kept (acc may be NULL) */
+#define B2_AGG_AND    5   /* bitwise AND / OR / XOR of int64 or B2_U8 (0/1) inputs; a B2_F64 input is B2_ERR_ARG */
+#define B2_AGG_OR     6
+#define B2_AGG_XOR    7
 
 /* join flags */
 #define B2_JOIN_INNER        0
@@ -113,7 +116,7 @@ typedef struct b2_agg {
 } b2_agg_t;
 
 /* per-slot accumulators of a group table (caller-allocated, caller-initialised:
- * SUM/COUNT arrays 0, MIN arrays INT64_MAX, MAX arrays INT64_MIN).
+ * SUM/COUNT/OR/XOR arrays 0, MIN arrays INT64_MAX, MAX arrays INT64_MIN, AND arrays -1 (all ones)).
  * float64 MIN/MAX accumulators hold the order-preserving int64 image of the double
  * (see b2_f64_to_ordered in DESIGN.md); b2_ordered_to_f64() converts back. */
 typedef struct b2_aggstate {
@@ -280,9 +283,10 @@ int32_t b2_groupby_hashk(const b2_scan_t* scan, const int32_t* key_cols, int32_t
                          int64_t cap, const b2_agg_t* aggs, int32_t naggs,
                          const b2_aggstate_t* st, int32_t* d_flags, void* stream);
 
-/* dst |= src over nwords 32-bit words: merges the presence bitmaps of per-GPU dense group tables
- * after an all-gather (NCCL has no bitwise reduction). */
-int32_t b2_bitmap_or(uint32_t* dst, const uint32_t* src, int64_t nwords, void* stream);
+/* dst = dst <op> src over nwords 32-bit words, op = B2_AGG_AND / B2_AGG_OR / B2_AGG_XOR.  NCCL has no
+ * bitwise reduction: this folds the slot chunks of per-GPU dense group tables after an all-to-all (a
+ * bitwise op on 64-bit accumulators is the same op on their two 32-bit halves). */
+int32_t b2_bitwise_combine(uint32_t* dst, const uint32_t* src, int64_t nwords, int32_t op, void* stream);
 
 /* ---- multi-GPU merge of dense partial tables over NVLink peer memory ----------------------
  * Replaces dask's tree reduction of per-partition partial aggregates (aggregate.py:575-581,
@@ -307,6 +311,9 @@ int32_t b2_bitmap_or(uint32_t* dst, const uint32_t* src, int64_t nwords, void* s
 #define B2_PEER_SUM_I64 1   /* wraps (two's complement), like the single-GPU accumulators */
 #define B2_PEER_MIN_I64 2   /* MIN / MAX accumulators hold int64 values or ordered images of doubles */
 #define B2_PEER_MAX_I64 3
+#define B2_PEER_AND_I64 4   /* bitwise accumulators (B2_AGG_AND / OR / XOR) */
+#define B2_PEER_OR_I64  5
+#define B2_PEER_XOR_I64 6
 #define B2_PEER_PRESENT_ROWS      1   /* group exists iff merged array[presence_array] > 0 */
 #define B2_PEER_PRESENT_INDICATOR 2   /* ... iff some rank's array[presence_array] bits != B2_EMPTY_KEY (-0.0) */
 #define B2_PEER_PRESENT_BITMAP    3   /* ... iff some rank's bitmap bit is set */

@@ -91,6 +91,24 @@ def main():
     got = c.sql("""SELECT d.grp, MIN(f.x) AS lo FROM fact f JOIN dim d ON f.fk = d.pk
                    WHERE d.flag < 5 GROUP BY d.grp""", return_futures=False)
     check(got, e.groupby("grp", dropna=False).agg(lo=("x", "min")).reset_index(), ["grp"], [], ["lo"])
+    # bitwise accumulators: AND / OR / XOR merged by the peer kernel, and by all-to-all + b2_bitwise_combine
+    # under NCCL (which has no bitwise reduction)
+    qb = """SELECT d.grp, BIT_AND(f.x) AS ba, BIT_OR(f.x) AS bo, BIT_XOR(f.x) AS bx FROM fact f JOIN dim d
+            ON f.fk = d.pk WHERE d.flag < 5 GROUP BY d.grp"""
+    bits = e.groupby("grp", dropna=False).x
+    expb = pd.DataFrame({"grp": bits.apply(lambda s: 0).index,
+                         "ba": bits.apply(lambda s: np.bitwise_and.reduce(s.to_numpy())).values,
+                         "bo": bits.apply(lambda s: np.bitwise_or.reduce(s.to_numpy())).values,
+                         "bx": bits.apply(lambda s: np.bitwise_xor.reduce(s.to_numpy())).values})
+    for rep in range(3):
+        check(c.sql(qb, return_futures=False), expb, ["grp"], [], ["ba", "bo", "bx"])
+    os.environ["B200SQL_PEER_MERGE"] = "0"
+    c4 = Context()
+    c4.create_table("fact", fact.iloc[lo:hi], persist=True, npartitions=3, distribution="sharded")
+    c4.create_table("dim", dim if rank == 0 else dim.iloc[:0], persist=True, distribution="root")
+    for rep in range(2):
+        check(c4.sql(qb, return_futures=False), expb, ["grp"], [], ["ba", "bo", "bx"])
+    del os.environ["B200SQL_PEER_MERGE"]
     # 1c. composite group key on the build side: hashed slots differ per rank -> merged by key
     got = c.sql("""SELECT d.grp, d.flag, SUM(f.val) AS rev, COUNT(*) AS n FROM fact f JOIN dim d ON f.fk = d.pk
                    WHERE f.x > 0 GROUP BY d.grp, d.flag""", return_futures=False)

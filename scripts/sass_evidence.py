@@ -20,8 +20,8 @@ WANT = {
     "groupby_dense": r"b2_groupby_dense_kernelILb0E",
     "groupby_dense_hh": r"b2_groupby_dense_hh_kernel",
     "groupby_dense_grouped": r"b2_groupby_dense_grouped_kernel",
-    "scan_agg": r"b2_scan_agg_kernelILb0E",
-    "scan_agg_tma": r"b2_scan_agg_kernelILb1E",
+    "scan_agg": r"b2_scan_agg_kernelILb0ELb0E",
+    "scan_agg_tma": r"b2_scan_agg_kernelILb1ELb0E",
 }
 INTERESTING = re.compile(r"\b(LDG|STG|REDG|ATOMG|ATOMS|ATOM|RED|LDS|STS|MATCH|VOTE|SHFL|REDUX|UBLKCP|SYNCS|BAR|CCTL|LDGSTS|UTMALDG|LD|ST|NANOSLEEP|MEMBAR|ERRBAR)\b")
 
