@@ -73,7 +73,7 @@ class JoinAgg(C.Structure):
 
 
 class StarLookup(C.Structure):
-    _fields_ = [("dense", C.c_int32), ("pad_", C.c_int32), ("lookup", C.c_void_p), ("kmin", C.c_int64),
+    _fields_ = [("dense", C.c_int32), ("slot_bits", C.c_int32), ("lookup", C.c_void_p), ("kmin", C.c_int64),
                 ("range", C.c_int64), ("table_keys", C.c_void_p), ("table_slots", C.c_void_p),
                 ("cap", C.c_int64), ("dir", C.c_void_p)]
 
@@ -193,6 +193,8 @@ _SIGS = {
     "b2_star_build_rank": [_P, C.c_int64, _P],
     "b2_star_build_fill": [C.POINTER(Scan), C.c_int32, C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_int32, _P,
                            _P, _P],
+    "b2_star_build_fill_packed": [C.POINTER(Scan), C.c_int32, C.c_int32, C.c_int64, C.c_int64, C.c_int64,
+                                  C.c_int32, _P, _P, C.c_int32, _P],
     "b2_star_build_hash": [C.POINTER(Col), _P, C.c_int64, _P, _P, _P, C.c_int64, _P, _P],
     "b2_star_agg": [C.POINTER(Scan), C.c_int32, C.POINTER(StarLookup), C.POINTER(Agg), C.c_int32,
                     C.POINTER(AggState), _P],
@@ -283,6 +285,7 @@ star_build_dense = _wrap("b2_star_build_dense")
 star_build_mark = _wrap("b2_star_build_mark")
 star_build_rank = _wrap("b2_star_build_rank")
 star_build_fill = _wrap("b2_star_build_fill")
+star_build_fill_packed = _wrap("b2_star_build_fill_packed")
 star_build_hash = _wrap("b2_star_build_hash")
 star_agg = _wrap("b2_star_agg")
 num_tiles = _lib.b2_num_tiles

@@ -274,11 +274,19 @@ b2_star_build_dense_kernel(const __grid_constant__ b2_col_t pk, const int32_t* _
 //   rank  (once): exclusive scan of the words' popcounts into their rank fields;
 //   FILL  (every partition): predicate again -> slots[rank + set bits below the key's] = group slot.
 // The rank is global, so every partition's MARK must precede the scan.
+//
+// The slots are packed `slot_bits` (16, 21 or 32) wide, k = 64 / slot_bits to a 64-bit word, none
+// crossing a word: entry i is bits [(i mod k) * slot_bits, + slot_bits) of word i / k.  32 bits is
+// a plain int32 array.  b2_slot_word is the only place that divides by k.
+__device__ __forceinline__ uint32_t b2_slot_word(uint32_t pos, int slot_bits) {
+  return slot_bits == 16 ? pos >> 2 : __umulhi(pos, 0x55555556u);   // pos / 3, exact for pos < 2^31
+}
+
 template <bool FILL>
 __global__ void __launch_bounds__(B2_BLOCK)
 b2_star_build_scan_kernel(const __grid_constant__ b2_scan_t s, int pk_col, int grp_col, int64_t pk_min,
                           int64_t pk_range, int64_t grp_min, int32_t null_slot, uint64_t* __restrict__ dir,
-                          int32_t* __restrict__ slots, int32_t* __restrict__ flags) {
+                          void* __restrict__ slots, int slot_bits, int32_t* __restrict__ flags) {
   const int tile_off = (threadIdx.x >> 5) * (32 * B2_GB_R) + (threadIdx.x & 31);
   const b2_col_t& pc = s.cols[pk_col];
   const b2_col_t& gc = s.cols[grp_col];
@@ -315,7 +323,23 @@ b2_star_build_scan_kernel(const __grid_constant__ b2_scan_t s, int pk_col, int g
         const uint64_t d = (uint64_t)pk[j] - (uint64_t)pk_min;
         const uint64_t w = dir[d >> 5];
         const uint32_t pos = (uint32_t)(w >> 32) + __popc((uint32_t)w & ((1u << (d & 31)) - 1));
-        slots[pos] = (gnull >> j) & 1 ? null_slot : (int32_t)(grp[j] - grp_min);
+        const int32_t v = (gnull >> j) & 1 ? null_slot : (int32_t)(grp[j] - grp_min);
+        if (slot_bits == 32) {
+          static_cast<int32_t*>(slots)[pos] = v;
+        } else {
+          // The k entries of a word come from different dim rows, so the word is updated atomically, and
+          // the entry is REPLACED, not ORed in: two passing rows with the same pk share one directory bit
+          // and so one entry, and an OR of their slots could exceed null_slot and send the probe's atomics
+          // past the group table before the host reads the duplicate flag.  As with the 32-bit store, one
+          // of the two valid slots wins.  The first guess is the zeroed word.
+          const uint32_t q = b2_slot_word(pos, slot_bits);
+          const uint32_t sh = (pos - q * (64 / slot_bits)) * slot_bits;
+          unsigned long long* p = reinterpret_cast<unsigned long long*>(slots) + q;
+          const unsigned long long m = ((1ull << slot_bits) - 1) << sh;
+          const unsigned long long e = ((unsigned long long)(uint32_t)v << sh) & m;
+          unsigned long long old = 0, seen;
+          while ((seen = atomicCAS(p, old, (old & ~m) | e)) != old) old = seen;
+        }
       }
     }
   }
@@ -393,6 +417,7 @@ __device__ __forceinline__ void b2_star_body(const b2_scan_t& s, const LD& ld, i
   const bool prefetch = aggs.n > 0 && aggs.a[0].col >= 0;
   int64_t pre[R];   // only read when `prefetch`: otherwise aggregate 0 has no input column, or is absent
   int32_t found[R];
+  int64_t slot[R];
   if (lk.dense == 2) {
     // ranked bitmap: every directory word first, then the slot reads for the keys whose bit is set.
     // The prefetch is issued between the two so that it stays in flight across both round trips.
@@ -404,11 +429,38 @@ __device__ __forceinline__ void b2_star_body(const b2_scan_t& s, const LD& ld, i
       w[j] = (((live >> j) & 1) && d < range) ? (uint64_t)b2_ld_keep_i64(reinterpret_cast<const int64_t*>(lk.dir) + (d >> 5)) : 0;
     }
     if (prefetch) ld.template load<R>(aggs.a[0].col, live, false, pre);
+    const int sb = lk.slot_bits;   // 16, 21 or 32 (b2_star_agg normalises 0); uniform across the grid
+    if (sb == 32) {
+      // never a 64-bit read here: with an odd entry count it would run 4 bytes past the array
 #pragma unroll
-    for (int j = 0; j < R; ++j) {
-      const uint32_t b = (uint32_t)((uint64_t)key[j] - (uint64_t)lk.kmin) & 31;
-      const uint32_t bits = (uint32_t)w[j];
-      found[j] = (bits >> b) & 1 ? b2_ld_keep_i32(lk.lookup + (uint32_t)(w[j] >> 32) + __popc(bits & ((1u << b) - 1))) : -1;
+      for (int j = 0; j < R; ++j) {
+        const uint32_t b = (uint32_t)((uint64_t)key[j] - (uint64_t)lk.kmin) & 31;
+        const uint32_t bits = (uint32_t)w[j];
+        found[j] = (bits >> b) & 1 ? b2_ld_keep_i32(lk.lookup + (uint32_t)(w[j] >> 32) + __popc(bits & ((1u << b) - 1))) : -1;
+      }
+    } else {
+      // packed: slot[j] holds the loaded word until it is decoded, found[j] the entry's shift (-1: no
+      // partner).  The decoded slot goes to found[j]: kept 32 bits wide it costs the aggregation that
+      // follows 16 fewer registers than a 64-bit one.
+      const int k = 64 / sb;
+      const uint64_t* words = reinterpret_cast<const uint64_t*>(lk.lookup);
+#pragma unroll
+      for (int j = 0; j < R; ++j) {
+        const uint32_t b = (uint32_t)((uint64_t)key[j] - (uint64_t)lk.kmin) & 31;
+        const uint32_t bits = (uint32_t)w[j];
+        found[j] = -1;
+        slot[j] = 0;
+        if ((bits >> b) & 1) {
+          const uint32_t pos = (uint32_t)(w[j] >> 32) + __popc(bits & ((1u << b) - 1));
+          const uint32_t q = b2_slot_word(pos, sb);
+          found[j] = (int32_t)((pos - q * k) * sb);
+          slot[j] = b2_ld_keep_i64(reinterpret_cast<const int64_t*>(words + q));
+        }
+      }
+      const uint64_t mask = (1ull << sb) - 1;
+#pragma unroll
+      for (int j = 0; j < R; ++j)
+        found[j] = found[j] < 0 ? -1 : (int32_t)(((uint64_t)slot[j] >> found[j]) & mask);
     }
   } else if (lk.dense) {
     const uint64_t range = (uint64_t)lk.range;
@@ -425,7 +477,6 @@ __device__ __forceinline__ void b2_star_body(const b2_scan_t& s, const LD& ld, i
     }
   }
   if (lk.dense != 2 && prefetch) ld.template load<R>(aggs.a[0].col, live, false, pre);
-  int64_t slot[R];
 #pragma unroll
   for (int j = 0; j < R; ++j) slot[j] = found[j];
   // `pre` is passed as it is, never as a pointer chosen at run time: that would put it in local memory
@@ -649,7 +700,7 @@ int32_t b2_star_build_dense(const b2_col_t* pk, const int32_t* sel, int64_t n_se
 
 static int32_t b2_star_build_pass(bool fill, const b2_scan_t* scan, int32_t pk_col, int32_t grp_col,
                                   int64_t pk_min, int64_t pk_range, int64_t grp_min, int32_t null_slot,
-                                  uint64_t* dir, int32_t* slots, int32_t* d_flags, void* stream) {
+                                  uint64_t* dir, void* slots, int32_t slot_bits, int32_t* d_flags, void* stream) {
   int32_t rc = b2_check_scan(scan);
   if (rc) return rc;
   B2_REQUIRE(pk_col >= 0 && pk_col < scan->ncols && grp_col >= 0 && grp_col < scan->ncols, "column out of range");
@@ -660,11 +711,11 @@ static int32_t b2_star_build_pass(bool fill, const b2_scan_t* scan, int32_t pk_c
   if (fill) {
     int grid = b2_wave_grid(b2_star_build_scan_kernel<true>, B2_BLOCK, nblk);
     b2_star_build_scan_kernel<true><<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(*scan, pk_col, grp_col, pk_min, pk_range,
-                                                                                  grp_min, null_slot, dir, slots, d_flags);
+                                                                                  grp_min, null_slot, dir, slots, slot_bits, d_flags);
   } else {
     int grid = b2_wave_grid(b2_star_build_scan_kernel<false>, B2_BLOCK, nblk);
     b2_star_build_scan_kernel<false><<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(*scan, pk_col, grp_col, pk_min, pk_range,
-                                                                                   grp_min, null_slot, dir, slots, d_flags);
+                                                                                   grp_min, null_slot, dir, slots, slot_bits, d_flags);
   }
   B2_CHECK_LAUNCH("b2_star_build_scan_kernel");
   return B2_OK;
@@ -673,7 +724,7 @@ static int32_t b2_star_build_pass(bool fill, const b2_scan_t* scan, int32_t pk_c
 int32_t b2_star_build_mark(const b2_scan_t* scan, int32_t pk_col, int64_t pk_min, int64_t pk_range, uint64_t* dir,
                            int32_t* d_flags, void* stream) {
   B2_REQUIRE(dir && d_flags, "null argument");
-  return b2_star_build_pass(false, scan, pk_col, pk_col, pk_min, pk_range, 0, 0, dir, nullptr, d_flags, stream);
+  return b2_star_build_pass(false, scan, pk_col, pk_col, pk_min, pk_range, 0, 0, dir, nullptr, 32, d_flags, stream);
 }
 
 int32_t b2_star_build_rank(uint64_t* dir, int64_t pk_range, void* stream) {
@@ -687,9 +738,19 @@ int32_t b2_star_build_rank(uint64_t* dir, int64_t pk_range, void* stream) {
 int32_t b2_star_build_fill(const b2_scan_t* scan, int32_t pk_col, int32_t grp_col, int64_t pk_min,
                            int64_t pk_range, int64_t grp_min, int32_t null_slot, const uint64_t* dir,
                            int32_t* slots, void* stream) {
+  return b2_star_build_fill_packed(scan, pk_col, grp_col, pk_min, pk_range, grp_min, null_slot, dir,
+                                   reinterpret_cast<uint64_t*>(slots), 32, stream);
+}
+
+int32_t b2_star_build_fill_packed(const b2_scan_t* scan, int32_t pk_col, int32_t grp_col, int64_t pk_min,
+                                  int64_t pk_range, int64_t grp_min, int32_t null_slot, const uint64_t* dir,
+                                  uint64_t* slots, int32_t slot_bits, void* stream) {
   B2_REQUIRE(dir && slots, "null argument");
+  B2_REQUIRE(slot_bits == 16 || slot_bits == 21 || slot_bits == 32, "slot_bits must be 16, 21 or 32");
+  B2_REQUIRE(slot_bits == 32 || (null_slot >= 0 && null_slot < (1 << slot_bits)), "null_slot does not fit slot_bits");
+  B2_REQUIRE(slot_bits == 32 || ((uintptr_t)slots & 7) == 0, "packed slots must be 8-byte aligned");
   return b2_star_build_pass(true, scan, pk_col, grp_col, pk_min, pk_range, grp_min, null_slot,
-                            const_cast<uint64_t*>(dir), slots, nullptr, stream);
+                            const_cast<uint64_t*>(dir), slots, slot_bits, nullptr, stream);
 }
 
 int32_t b2_star_build_hash(const b2_col_t* pk, const int32_t* sel, int64_t n_sel, const int32_t* slot_of_row,
@@ -717,19 +778,25 @@ int32_t b2_star_agg(const b2_scan_t* scan, int32_t fk_col, const b2_starlookup_t
   B2_REQUIRE(fk_col >= 0 && fk_col < scan->ncols, "fk column out of range");
   B2_REQUIRE(scan->cols[fk_col].dtype == B2_I64, "fk must be int64");
   B2_REQUIRE(lk->dense >= 0 && lk->dense <= 2, "bad lookup kind");
-  if (lk->dense == 2) B2_REQUIRE(lk->dir && lk->lookup && lk->range > 0 && lk->range < ((int64_t)1 << 31), "bad bitmap lookup");
-  else if (lk->dense) B2_REQUIRE(lk->lookup && lk->range > 0, "bad dense lookup");
-  else B2_REQUIRE(lk->table_keys && lk->table_slots && b2_pow2(lk->cap), "bad hash lookup");
+  b2_starlookup_t l = *lk;
+  if (l.dense == 2) {
+    B2_REQUIRE(l.dir && l.lookup && l.range > 0 && l.range < ((int64_t)1 << 31), "bad bitmap lookup");
+    if (l.slot_bits == 0) l.slot_bits = 32;
+    B2_REQUIRE(l.slot_bits == 16 || l.slot_bits == 21 || l.slot_bits == 32, "slot_bits must be 0, 16, 21 or 32");
+    B2_REQUIRE(l.slot_bits == 32 || ((uintptr_t)l.lookup & 7) == 0, "packed slots must be 8-byte aligned");
+  }
+  else if (l.dense) B2_REQUIRE(l.lookup && l.range > 0, "bad dense lookup");
+  else B2_REQUIRE(l.table_keys && l.table_slots && b2_pow2(l.cap), "bad hash lookup");
   if (scan->n == 0) return B2_OK;
   b2_pipe_t pp;
   b2_make_pipe(*scan, &pp);
   if (pp.enabled) {
     int grid = b2_pipe_grid(b2_star_agg_kernel<true>, pp, scan->n);
-    b2_star_agg_kernel<true><<<grid, B2_PIPE_THREADS, pp.smem_bytes, (cudaStream_t)stream>>>(*scan, pp, fk_col, *lk, aa, *st);
+    b2_star_agg_kernel<true><<<grid, B2_PIPE_THREADS, pp.smem_bytes, (cudaStream_t)stream>>>(*scan, pp, fk_col, l, aa, *st);
   } else {
     int64_t nblk = (scan->n + (int64_t)B2_BLOCK * B2_STAR_R - 1) / ((int64_t)B2_BLOCK * B2_STAR_R);
     int grid = b2_wave_grid(b2_star_agg_kernel<false>, B2_BLOCK, nblk);
-    b2_star_agg_kernel<false><<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(*scan, pp, fk_col, *lk, aa, *st);
+    b2_star_agg_kernel<false><<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(*scan, pp, fk_col, l, aa, *st);
   }
   B2_CHECK_LAUNCH("b2_star_agg_kernel");
   return B2_OK;

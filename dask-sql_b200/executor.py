@@ -1715,9 +1715,10 @@ class PreparedStar:
         # alternating buffers would keep both sets of evict_last lines next to the group tables, and a step
         # would meet a lookup that the other buffer's protected lines have displaced.)
         self.dn = dn
-        _, self.flags_off, words = _star_bitmap_words(self.prange, dn)
+        self.slot_bits = _star_slot_bits(self.nslots - 1)
+        _, self.flags_off, words = _star_bitmap_words(self.prange, dn, self.slot_bits)
         self.lookup = torch.empty(words, dtype=torch.int32, device=dev)
-        self.lk = _star_bitmap_lookup(self.lookup, self.pmin, self.prange, dn)
+        self.lk = _star_bitmap_lookup(self.lookup, self.pmin, self.prange, dn, self.slot_bits)
         # group tables: ONE (re-initialised per run) on the NCCL / single-GPU path; enable_peer_merge()
         # replaces it with two in symmetric memory that alternate run by run
         self.tabs = [GroupState(dev, self.nslots, self.plan, need_present=True,
@@ -1860,7 +1861,7 @@ class PreparedStar:
         if self.owner:
             with _Phase("build"):
                 _star_bitmap_build(buf, self.dim_launch, self.pmin, self.prange, self.gmin, self.nslots - 1,
-                                   self.dn, sp)
+                                   self.dn, self.slot_bits, sp)
         if self.bcast:
             with _Phase("bcast"):
                 P.broadcast_(buf, 0)
@@ -1906,30 +1907,40 @@ class _NotPreparable(Exception):
     pass
 
 
-def _star_bitmap_words(prange, dn):
+def _star_slot_bits(null_slot):
+    """Width of the packed slots of a ranked-bitmap star lookup (include/b200sql.h, b2_star_build_mark):
+    the narrowest of 16, 21 and 32 bits that holds the largest slot, null_slot.  Narrower slots keep
+    more of the lookup in L2 while the fact columns stream past."""
+    return 16 if null_slot < (1 << 16) else 21 if null_slot < (1 << 21) else 32
+
+
+def _star_bitmap_words(prange, dn, slot_bits):
     """int32 offsets within the one buffer of a ranked-bitmap star lookup (include/b200sql.h,
     b2_star_build_mark): (slots, flags, total).  The directory comes first, two words per 32 keys; the
-    slots hold one entry per set bit, at most one per dim row and one per key; 4 flag words close it.
-    One buffer, so that a 'root' table's lookup crosses to the other ranks in one broadcast."""
+    slots hold one entry per set bit, at most one per dim row and one per key, 64 // slot_bits to a
+    64-bit word (so they start and end 8-byte aligned); 4 flag words close it.  One buffer, so that a
+    'root' table's lookup crosses to the other ranks in one broadcast."""
     slots = 2 * ((prange + 31) // 32)
-    flags = slots + min(dn, prange)
+    k = 64 // slot_bits
+    flags = slots + 2 * ((min(dn, prange) + k - 1) // k)
     return slots, flags, flags + 4
 
 
-def _star_bitmap_lookup(buf, pmin, prange, dn):
+def _star_bitmap_lookup(buf, pmin, prange, dn, slot_bits):
     lk = L.StarLookup()
-    lk.dense, lk.dir, lk.kmin, lk.range = 2, buf.data_ptr(), pmin, prange
-    lk.lookup = buf.data_ptr() + 4 * _star_bitmap_words(prange, dn)[0]
+    lk.dense, lk.dir, lk.kmin, lk.range, lk.slot_bits = 2, buf.data_ptr(), pmin, prange, slot_bits
+    lk.lookup = buf.data_ptr() + 4 * _star_bitmap_words(prange, dn, slot_bits)[0]
     return lk
 
 
-def _star_bitmap_build(buf, launches, pmin, prange, gmin, null_slot, dn, sp):
+def _star_bitmap_build(buf, launches, pmin, prange, gmin, null_slot, dn, slot_bits, sp):
     """The ranked-bitmap lookup from (scan, pk slot, grp slot) of every dim partition, in stream order:
-    zero the directory and flags, mark every partition, rank, fill every partition."""
-    slots_off, flags_off, _ = _star_bitmap_words(prange, dn)
+    zero the directory (with packed slots, the slot words too: FILL ORs into them) and flags, mark every
+    partition, rank, fill every partition."""
+    slots_off, flags_off, _ = _star_bitmap_words(prange, dn, slot_bits)
     base = buf.data_ptr()
     dirp, slots, flags = C.c_void_p(base), C.c_void_p(base + 4 * slots_off), C.c_void_p(base + 4 * flags_off)
-    L.memset(dirp, 0, 4 * slots_off, sp)
+    L.memset(dirp, 0, 4 * (flags_off if slot_bits < 32 else slots_off), sp)
     L.memset(flags, 0, 16, sp)
     for scan, pk_slot, _ in launches:
         stats["launches"] += 1
@@ -1938,7 +1949,8 @@ def _star_bitmap_build(buf, launches, pmin, prange, gmin, null_slot, dn, sp):
     L.star_build_rank(dirp, prange, sp)
     for scan, pk_slot, g_slot in launches:
         stats["launches"] += 1
-        L.star_build_fill(C.byref(scan), pk_slot, g_slot, pmin, prange, gmin, null_slot, dirp, slots, sp)
+        L.star_build_fill_packed(C.byref(scan), pk_slot, g_slot, pmin, prange, gmin, null_slot, dirp, slots,
+                                 slot_bits, sp)
 
 
 def _star_dense_fast(src, fact, dim, fk_e, pk_e, gexprs, aggs, fact_pred, dim_pred, sharded, dev) -> Optional[Part]:
@@ -1989,7 +2001,8 @@ def _star_dense_fast(src, fact, dim, fk_e, pk_e, gexprs, aggs, fact_pred, dim_pr
         if prep is not None:
             return prep.run(src)
     # directory, slots and the 4 flag words share one buffer: one broadcast carries them all
-    _, flags_off, words = _star_bitmap_words(prange, dn)
+    slot_bits = _star_slot_bits(nslots - 1)
+    _, flags_off, words = _star_bitmap_words(prange, dn, slot_bits)
     buf = torch.empty(words, dtype=torch.int32, device=dev)
     flags = buf[flags_off:]
     with _Phase("build"):
@@ -2005,7 +2018,7 @@ def _star_dense_fast(src, fact, dim, fk_e, pk_e, gexprs, aggs, fact_pred, dim_pr
                 pk_slot, g_slot = ctx.slot(pk_e), ctx.slot(ge)     # slots first: scan() snapshots the columns
                 launches.append((ctx.scan(), pk_slot, g_slot))
                 keep.append(ctx)
-            _star_bitmap_build(buf, launches, pmin, prange, gmin, nslots - 1, dn, D.stream_ptr())
+            _star_bitmap_build(buf, launches, pmin, prange, gmin, nslots - 1, dn, slot_bits, D.stream_ptr())
     if world > 1 and dist == "root":
         # the build side crosses NVLink as the finished lookup (directory + slots), not as its columns
         with _Phase("bcast"):
@@ -2013,7 +2026,7 @@ def _star_dense_fast(src, fact, dim, fk_e, pk_e, gexprs, aggs, fact_pred, dim_pr
     plan = AggPlan([(E.substitute(e, fact.exprs) if e is not None else None, o, f) for e, o, f in aggs],
                    _nullable_fn(fact, sharded))
     gs = GroupState(dev, nslots, plan, need_present=True, alloc=_padded_slots(nslots, sharded))
-    lk = _star_bitmap_lookup(buf, pmin, prange, dn)
+    lk = _star_bitmap_lookup(buf, pmin, prange, dn, slot_bits)
     needed = set(fk_e.refs())
     for ka in plan.kaggs:
         ka.expr.refs(needed)

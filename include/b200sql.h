@@ -524,16 +524,24 @@ int32_t b2_star_build_dense(const b2_col_t* pk, const int32_t* sel, int64_t n_se
  *   dir   = uint64[(pk_range + 31) / 32]: bits (low half) = one bit per key of [pk_min, pk_min + pk_range)
  *           whose build row passes the terms and has a non-NULL key; rank (high half) = set bits in all
  *           earlier words;
- *   slots = int32[min(build rows, pk_range)]: one entry per set bit in key order, grp - grp_min
- *           (NULL grp -> null_slot).
- * In stream order: zero dir; b2_star_build_mark on every build partition (d_flags[0] = 1 on a duplicate
- * pk among the rows that pass); b2_star_build_rank once; b2_star_build_fill on every build partition. */
+ *   slots = min(build rows, pk_range) entries, one per set bit in key order, grp - grp_min (NULL grp ->
+ *           null_slot), each slot_bits wide: k = 64 / slot_bits entries to a little-endian uint64 word,
+ *           none crossing a word, entry i at bit (i mod k) * slot_bits of word i / k; unused bits are 0.
+ *           slot_bits = 16 (null_slot < 2^16, k = 4), 21 (null_slot < 2^21, k = 3), else 32 (k = 2),
+ *           which is exactly an int32 array.
+ * In stream order: zero dir (and, below 32 bits, the slot words); b2_star_build_mark on every build
+ * partition (d_flags[0] = 1 on a duplicate pk among the rows that pass); b2_star_build_rank once;
+ * b2_star_build_fill_packed on every build partition.  b2_star_build_fill is its 32-bit case, which
+ * stores every entry it owns and needs no zeroed slots. */
 int32_t b2_star_build_mark(const b2_scan_t* scan, int32_t pk_col, int64_t pk_min, int64_t pk_range,
                            uint64_t* dir, int32_t* d_flags, void* stream);
 int32_t b2_star_build_rank(uint64_t* dir, int64_t pk_range, void* stream);
 int32_t b2_star_build_fill(const b2_scan_t* scan, int32_t pk_col, int32_t grp_col, int64_t pk_min,
                            int64_t pk_range, int64_t grp_min, int32_t null_slot, const uint64_t* dir,
                            int32_t* slots, void* stream);
+int32_t b2_star_build_fill_packed(const b2_scan_t* scan, int32_t pk_col, int32_t grp_col, int64_t pk_min,
+                                  int64_t pk_range, int64_t grp_min, int32_t null_slot, const uint64_t* dir,
+                                  uint64_t* slots, int32_t slot_bits, void* stream);
 /* Hash variant: table_keys = int64[cap] pre-filled with B2_EMPTY_KEY, table_slots = int32[cap].
  * d_flags[0] = 1 on duplicate pk, d_flags[1] = 1 on overflow. */
 int32_t b2_star_build_hash(const b2_col_t* pk, const int32_t* sel, int64_t n_sel,
@@ -542,8 +550,8 @@ int32_t b2_star_build_hash(const b2_col_t* pk, const int32_t* sel, int64_t n_sel
 
 typedef struct b2_starlookup {
   int32_t dense;           /* 0: hash table, 1: int32 per key, 2: ranked bitmap (b2_star_build_mark) */
-  int32_t pad_;
-  const int32_t* lookup;   /* 1: int32[range], -1 = no partner; 2: the slots array */
+  int32_t slot_bits;       /* 2: width of the slots, 16, 21 or 32; 0 means 32 */
+  const int32_t* lookup;   /* 1: int32[range], -1 = no partner; 2: the slots array (8-byte aligned below 32 bits) */
   int64_t kmin;
   int64_t range;
   const int64_t* table_keys;  /* hash */
