@@ -25,6 +25,10 @@ OP_ADD_I, OP_SUB_I, OP_MUL_I, OP_DIV_I, OP_NEG_I, OP_ABS_I, OP_MOD_I = 10, 11, 1
 OP_ADD_F, OP_SUB_F, OP_MUL_F, OP_DIV_F, OP_NEG_F, OP_ABS_F, OP_SQRT_F = 20, 21, 22, 23, 24, 25, 26
 OP_EQ_I, OP_EQ_F = 30, 40
 OP_AND, OP_OR, OP_NOT, OP_ISNULL_I, OP_ISNULL_F, OP_CASE, OP_FILLNA, OP_ORD2F = 50, 51, 52, 53, 54, 55, 56, 57
+OP_DATEPART, OP_ADDMONTHS = 60, 61
+# B2_OP_DATEPART fields (b200sql.h B2_DP_*)
+(DP_DAYS, DP_YEAR, DP_QUARTER, DP_MONTH, DP_DAY, DP_DOY, DP_DOW, DP_ISOWEEK, DP_HOUR, DP_MINUTE, DP_SECOND,
+ DP_MILLISECOND, DP_MICROSECOND) = range(13)
 
 
 class Col(C.Structure):

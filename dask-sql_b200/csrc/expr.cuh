@@ -11,6 +11,81 @@ struct b2_cols_arg {
   b2_col_t c[B2_MAX_COLS];
 };
 
+// ---- calendar arithmetic (proleptic Gregorian, days since 1970-01-01) ---------------------
+// Howard Hinnant's civil_from_days / days_from_civil: int64 arithmetic with constant divisors only,
+// exact for every day an int64 tick count of any unit can reach (and the whole date32 range).
+__device__ __forceinline__ int64_t b2_floordiv(int64_t a, int64_t b) {  // b > 0
+  const int64_t q = a / b;
+  return q - (q * b > a);
+}
+
+__device__ __forceinline__ void b2_civil_from_days(int64_t z, int64_t& y, int& m, int& d) {
+  z += 719468;
+  const int64_t era = b2_floordiv(z, 146097);
+  const int64_t doe = z - era * 146097;                                       // [0, 146096]
+  const int64_t yoe = (doe - doe / 1460 + doe / 36524 - doe / 146096) / 365;  // [0, 399]
+  const int64_t doy = doe - (365 * yoe + yoe / 4 - yoe / 100);                // [0, 365], from March 1
+  const int64_t mp = (5 * doy + 2) / 153;                                     // [0, 11]
+  d = (int)(doy - (153 * mp + 2) / 5 + 1);
+  m = (int)(mp < 10 ? mp + 3 : mp - 9);
+  y = yoe + era * 400 + (m <= 2);
+}
+
+__device__ __forceinline__ int64_t b2_days_from_civil(int64_t y, int m, int d) {
+  y -= m <= 2;
+  const int64_t era = b2_floordiv(y, 400);
+  const int64_t yoe = y - era * 400;
+  const int64_t doy = (153 * (m > 2 ? m - 3 : m + 9) + 2) / 5 + d - 1;
+  const int64_t doe = yoe * 365 + yoe / 4 - yoe / 100 + doy;
+  return era * 146097 + doe - 719468;
+}
+
+// Kept out of line: the interpreter loop is walked by every instruction of every program, and the
+// calendar code would otherwise add its registers to all of them.
+__device__ __noinline__ int64_t b2_datepart(int64_t x, int field, int64_t tps) {
+  const int64_t tpd = tps ? tps * 86400 : 1;
+  const int64_t day = b2_floordiv(x, tpd);
+  const int64_t tod = x - day * tpd;
+  if (field == B2_DP_DAYS) return day;
+  if (field == B2_DP_DOW) return b2_floordiv(day + 4, 7) * -7 + day + 4;   // 1970-01-01 was a Thursday
+  if (field >= B2_DP_HOUR) {
+    if (!tps) return 0;
+    if (field == B2_DP_HOUR) return tod / (tps * 3600);
+    if (field == B2_DP_MINUTE) return tod / (tps * 60) % 60;
+    if (field == B2_DP_SECOND) return tod / tps % 60;
+    const int64_t sub = tod % tps;
+    return field == B2_DP_MILLISECOND ? sub * 1000 / tps : sub * 1000000 / tps;
+  }
+  int64_t y; int m, d;
+  if (field == B2_DP_ISOWEEK) {
+    // the ISO week belongs to the year of its Thursday
+    const int64_t th = day - (b2_floordiv(day + 3, 7) * -7 + day + 3) + 3;   // Mon = 0 .. Sun = 6
+    b2_civil_from_days(th, y, m, d);
+    return (th - b2_days_from_civil(y, 1, 1)) / 7 + 1;
+  }
+  b2_civil_from_days(day, y, m, d);
+  if (field == B2_DP_YEAR) return y;
+  if (field == B2_DP_QUARTER) return (m - 1) / 3 + 1;
+  if (field == B2_DP_MONTH) return m;
+  if (field == B2_DP_DAY) return d;
+  return day - b2_days_from_civil(y, 1, 1) + 1;                              // B2_DP_DOY
+}
+
+__device__ __noinline__ int64_t b2_addmonths(int64_t x, int64_t n, int64_t tps, int to_last) {
+  const int64_t tpd = tps ? tps * 86400 : 1;
+  const int64_t day = b2_floordiv(x, tpd);
+  const int64_t tod = x - day * tpd;
+  int64_t y; int m, d;
+  b2_civil_from_days(day, y, m, d);
+  const int64_t total = (int64_t)((uint64_t)(y * 12 + (m - 1)) + (uint64_t)n);
+  const int64_t y2 = b2_floordiv(total, 12);
+  const int m2 = (int)(total - y2 * 12) + 1;
+  const int64_t first = b2_days_from_civil(y2, m2, 1);
+  const int last = (int)(b2_days_from_civil(y2 + (m2 == 12), m2 == 12 ? 1 : m2 + 1, 1) - first);
+  const int d2 = to_last ? last : (d < last ? d : last);
+  return (int64_t)((uint64_t)(first + d2 - 1) * (uint64_t)tpd + (uint64_t)tod);
+}
+
 __global__ void __launch_bounds__(B2_BLOCK)
 b2_expr_kernel(const __grid_constant__ b2_prog_t prog, const __grid_constant__ b2_cols_arg cols,
                int64_t n, void* __restrict__ out_data, uint32_t* __restrict__ out_valid) {
@@ -74,6 +149,13 @@ b2_expr_kernel(const __grid_constant__ b2_prog_t prog, const __grid_constant__ b
         } else if (op == B2_OP_FILLNA) {
           // stack: x, fill
           if (sn[sp - 2]) { sv[sp - 2] = sv[sp - 1]; sn[sp - 2] = sn[sp - 1]; }
+          --sp;
+        } else if (op == B2_OP_DATEPART) {
+          sv[sp - 1] = b2_datepart(sv[sp - 1], ins.a, ins.imm_i);
+        } else if (op == B2_OP_ADDMONTHS) {
+          // stack: x, n
+          sv[sp - 2] = b2_addmonths(sv[sp - 2], sv[sp - 1], ins.imm_i, ins.a);
+          sn[sp - 2] = sn[sp - 2] || sn[sp - 1];
           --sp;
         } else {
           // binary operators: pops b then a
@@ -225,6 +307,19 @@ int32_t b2_expr_eval(const b2_prog_t* prog, const b2_col_t* cols, int32_t ncols,
     else if (op == B2_OP_I2F || op == B2_OP_F2I || op == B2_OP_NEG_I || op == B2_OP_ABS_I ||
              op == B2_OP_NEG_F || op == B2_OP_ABS_F || op == B2_OP_SQRT_F || op == B2_OP_NOT || op == B2_OP_ISNULL_I ||
              op == B2_OP_ISNULL_F || op == B2_OP_ORD2F) { B2_REQUIRE(sp >= 1, "stack underflow"); }
+    else if (op == B2_OP_DATEPART || op == B2_OP_ADDMONTHS) {
+      const int64_t tps = prog->code[i].imm_i;
+      B2_REQUIRE(tps == 0 || tps == 1 || tps == 1000 || tps == 1000000 || tps == 1000000000,
+                 "calendar opcode: ticks per second must be 0, 1, 10^3, 10^6 or 10^9");
+      if (op == B2_OP_DATEPART) {
+        B2_REQUIRE(prog->code[i].a >= 0 && prog->code[i].a < B2_DP_NFIELDS, "DATEPART: unknown field");
+        B2_REQUIRE(sp >= 1, "stack underflow");
+      } else {
+        B2_REQUIRE(prog->code[i].a == 0 || prog->code[i].a == 1, "ADDMONTHS: a must be 0 or 1");
+        B2_REQUIRE(sp >= 2, "stack underflow");
+        sp -= 1;
+      }
+    }
     else if (op == B2_OP_CASE) { B2_REQUIRE(sp >= 3, "stack underflow"); sp -= 2; }
     else { B2_REQUIRE(sp >= 2, "stack underflow"); sp -= 1; }
     B2_REQUIRE(sp <= B2_STACK, "expression too deep");

@@ -12,6 +12,7 @@ import numpy as np
 import torch
 
 from . import _lib as L
+from . import temporal as T
 from .expr import int_literal_is_exact
 
 I64, F64, U8 = L.I64, L.F64, L.U8
@@ -150,7 +151,10 @@ def column_from_host(values, device, pin=False) -> DeviceColumn:
     else:
         vals = np.asarray(values)
     kind = vals.dtype.kind
-    if kind == "b":
+    if kind == "M":               # DATE / TIMESTAMP: int64 ticks of the input's own unit, NaT -> NULL
+        vals, mask, logical = T.from_host_array(vals)
+        dt = I64
+    elif kind == "b":
         vals, dt = vals.astype(np.uint8), U8
     elif kind == "i" or (kind == "u" and vals.dtype.itemsize < 8):
         vals, dt = vals.astype(np.int64, copy=False), I64
@@ -184,6 +188,9 @@ def column_to_host(col: DeviceColumn):
         if not mask.any():
             mask = None
     lg = col.logical
+    unit = T.unit_of(lg)
+    if unit is not None:
+        return T.to_host_array(vals, unit, mask)
     if col.dtype == U8:
         vals = vals.astype(bool)
         if mask is not None or lg == "boolean":

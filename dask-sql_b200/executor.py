@@ -30,7 +30,6 @@ from .table import DeviceTable, HostColumn
 
 DENSE_MAX_SLOTS = 1 << 27          # direct-address group tables up to 128M slots
 _TORCH_DT = {I64: torch.int64, F64: torch.float64, U8: torch.uint8}
-_LOGICAL = {I64: "int64", F64: "float64", U8: "bool"}
 
 # counters the bench / tests read to prove which kernels ran
 stats = {"launches": 0, "star_fused": 0, "dense_groupby": 0, "hash_groupby": 0, "dense_join": 0,
@@ -258,7 +257,9 @@ def eval_expr(part: Part, e: Expr) -> DeviceColumn:
     prog = E.compile_expr(e, names)
     nullable = E.may_be_null(e, lambda n: part[n].valid is not None)
     stats["launches"] += 1
-    return D.expr_eval(prog, cols, part.n, nullable)
+    out = D.expr_eval(prog, cols, part.n, nullable)
+    out.logical = e.logical
+    return out
 
 
 def const_column(value, dtype, n, dev) -> DeviceColumn:
@@ -593,7 +594,7 @@ def empty_part(exprs: Dict[str, Expr]) -> Part:
     dev = _dev()
     out = Part({}, 0)
     for n, e in exprs.items():
-        lg = e.logical if isinstance(e, ColRef) else _LOGICAL[e.dtype]
+        lg = e.logical
         out[n] = DeviceColumn(torch.empty(0, dtype=_TORCH_DT[e.dtype], device=dev), None, e.dtype, lg)
     return out
 
@@ -625,6 +626,7 @@ def execute(frame: LazyFrame, needed: Optional[Sequence[str]] = None, top: bool 
         for n, e in exprs.items():
             if isinstance(e, Lit):
                 res[n] = const_column(e.value, e.dtype, part.n, _dev())
+                res[n].logical = e.logical
             else:
                 res[n] = eval_expr(part, e)
         return res
@@ -682,7 +684,7 @@ class AggPlan:
                 self.second[out] = self._slot(E.binop("mul", d, d), L.AGG_SUM, True)
                 self.outs.append((out, fn, a1, self._cnt(d), F64, "float64"))
                 continue
-            lg = (e.logical if isinstance(e, ColRef) else _LOGICAL[e.dtype]) if e is not None else "int64"
+            lg = e.logical if e is not None else "int64"
             if fn == "size" or e is None:
                 self.need_rows = True
                 self.outs.append((out, "size", None, "rows", I64, "int64"))
@@ -1016,7 +1018,7 @@ def grouped_aggregate(parts, pred, gexprs, gnames, plan: AggPlan, child, sharded
         total_rows_all = int(P.allreduce_(t).item())
     else:
         total_rows_all = total_rows
-    glog = [(e.logical if isinstance(e, ColRef) else _LOGICAL[e.dtype]) for e in gexprs]
+    glog = [e.logical for e in gexprs]
     if total_rows_all == 0:
         out = Part({}, 0)
         for g, e, lg in zip(gnames, gexprs, glog):
@@ -2125,7 +2127,7 @@ def try_star(src: AggSource, child: LazyFrame, gexprs, aggs, pred, sharded, allo
         return None
     plan = AggPlan([(E.substitute(e, fact.exprs) if e is not None else None, o, f) for e, o, f in aggs],
                    _nullable_fn(fact, sharded))
-    glog = [(e.logical if isinstance(e, ColRef) else _LOGICAL[e.dtype]) for e in gexprs]
+    glog = [e.logical for e in gexprs]
     glog = [dim.col_type(e.name)[1] if isinstance(e, ColRef) else l for e, l in zip(gexprs, glog)]
 
     # group slots of the dim rows

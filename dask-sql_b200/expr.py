@@ -10,6 +10,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import _lib as L
+from . import temporal as T
 
 I64, F64, U8 = L.I64, L.F64, L.U8
 _DT_NAME = {I64: "int64", F64: "float64", U8: "bool"}
@@ -30,6 +31,7 @@ def int_literal_is_exact(lit: float) -> bool:
 
 class Expr:
     dtype: int = I64
+    logical: str = "int64"
 
     def refs(self, out=None):
         out = set() if out is None else out
@@ -54,9 +56,11 @@ class ColRef(Expr):
 
 
 class Lit(Expr):
-    __slots__ = ("value", "dtype")
+    __slots__ = ("value", "dtype", "logical")
 
-    def __init__(self, value, dtype=None):
+    def __init__(self, value, dtype=None, logical=None):
+        if isinstance(value, T.TScalar):
+            value, dtype, logical = value.ticks, I64, value.logical
         if dtype is None:
             if value is None:
                 dtype = F64
@@ -69,24 +73,30 @@ class Lit(Expr):
             else:
                 raise NotImplementedError(f"literal {value!r} of type {type(value).__name__} is outside the "
                                           "int64/float64/bool hot path")
-        self.value, self.dtype = value, dtype
+        self.value, self.dtype, self.logical = value, dtype, logical or _DT_NAME[dtype]
 
     def __repr__(self):
+        if T.is_temporal(self.logical):
+            return f"lit({self.value!r}:{self.logical})"
         return f"lit({self.value!r})"
 
 
 class Call(Expr):
-    __slots__ = ("op", "args", "dtype")
+    """`param`: the static operand of an operator (the field of datepart, the to-last-day flag of
+    addmonths); `logical`: the result's logical dtype (a DATE / TIMESTAMP stays one through CASE, MIN ...)."""
+    __slots__ = ("op", "args", "dtype", "logical", "param")
 
-    def __init__(self, op, args, dtype):
+    def __init__(self, op, args, dtype, logical=None, param=None):
         self.op, self.args, self.dtype = op, tuple(args), dtype
+        self.logical, self.param = logical or _DT_NAME[dtype], param
 
     def _refs(self, out):
         for a in self.args:
             a._refs(out)
 
     def __repr__(self):
-        return f"{self.op}({', '.join(map(repr, self.args))})"
+        p = "" if self.param is None else f"[{self.param}]"
+        return f"{self.op}{p}({', '.join(map(repr, self.args))})"
 
 
 def as_expr(x) -> Expr:
@@ -95,6 +105,8 @@ def as_expr(x) -> Expr:
 
 def cast(e: Expr, dtype: int) -> Expr:
     if e.dtype == dtype:
+        if dtype == I64 and T.is_temporal(e.logical):     # a DATE / TIMESTAMP as BIGINT: its ticks
+            return Lit(e.value, I64) if isinstance(e, Lit) else Call("cast", [e], I64)
         return e
     if isinstance(e, Lit):
         if e.value is None:
@@ -111,7 +123,18 @@ def _arith_type(a: Expr, b: Expr):
     return F64 if F64 in (a.dtype, b.dtype) else I64
 
 
+def is_temporal(x) -> bool:
+    """A DATE / TIMESTAMP expression or host value, or an INTERVAL."""
+    return isinstance(x, (T.TScalar, T.Interval)) or (isinstance(x, Expr) and T.is_temporal(x.logical))
+
+
 def binop(op: str, a, b) -> Expr:
+    if is_temporal(a) or is_temporal(b):
+        return T.binop(op, a, b)
+    if op in _CMP:
+        r = T.rewrite_cmp(op, a, b)          # YEAR(x) <cmp> literal: a range on x
+        if r is not None:
+            return r
     a, b = as_expr(a), as_expr(b)
     if op in ("add", "sub", "mul", "mod"):
         t = _arith_type(a, b)
@@ -150,6 +173,9 @@ def unop(op: str, a) -> Expr:
 
 def case(cond, then, other) -> Expr:
     cond, then, other = as_expr(cond), as_expr(then), as_expr(other)
+    if is_temporal(then) or is_temporal(other):
+        then, other = T.unify(then, other)
+        return Call("case", [cast(cond, U8), then, other], I64, then.logical)
     if isinstance(then, Lit) and then.value is None:
         t = other.dtype
     elif isinstance(other, Lit) and other.value is None:
@@ -161,6 +187,9 @@ def case(cond, then, other) -> Expr:
 
 def fillna(a, fill) -> Expr:
     a, fill = as_expr(a), as_expr(fill)
+    if is_temporal(a) or is_temporal(fill):
+        a, fill = T.unify(a, fill)
+        return Call("fillna", [a, fill], I64, a.logical)
     return Call("fillna", [a, cast(fill, a.dtype)], a.dtype)
 
 
@@ -169,7 +198,7 @@ def substitute(e: Expr, mapping: Dict[str, Expr]) -> Expr:
     if isinstance(e, ColRef):
         return mapping[e.name]
     if isinstance(e, Call):
-        return Call(e.op, [substitute(a, mapping) for a in e.args], e.dtype)
+        return Call(e.op, [substitute(a, mapping) for a in e.args], e.dtype, e.logical, e.param)
     return e
 
 
@@ -330,6 +359,17 @@ class _Compiler:
         if op == "ord2f":
             self.visit(args[0])
             self.emit(L.OP_ORD2F)
+            return
+        if op == "datepart":
+            field, tps = e.param
+            self.visit(args[0])
+            self.emit(L.OP_DATEPART, a=field, imm_i=tps)
+            return
+        if op == "addmonths":
+            to_last, tps = e.param
+            self.visit(args[0])
+            self.visit(args[1])
+            self.emit(L.OP_ADDMONTHS, a=to_last, imm_i=tps)
             return
         raise NotImplementedError(f"expression operator {op}")
 

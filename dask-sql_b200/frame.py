@@ -19,6 +19,7 @@ from typing import Dict, List, Sequence
 import numpy as np
 
 from . import expr as E
+from . import temporal as T
 from .expr import Expr, ColRef, Lit, I64, F64, U8
 
 _NP_DTYPE = {I64: np.dtype("int64"), F64: np.dtype("float64"), U8: np.dtype("bool")}
@@ -82,6 +83,9 @@ class AggSource(Source):
                 self.schema[out] = (U8, "bool")
             else:
                 dt, lg = child.col_type(in_col)
+                if T.is_temporal(lg) and fn not in ("min", "max"):
+                    raise NotImplementedError(f"{fn.upper()} of a {T.sql_type_of(lg)} column: only COUNT, MIN and "
+                                              "MAX aggregate dates and timestamps")
                 if dt == U8:
                     dt, lg = I64, "int64"
                 self.schema[out] = (dt, lg)
@@ -115,6 +119,8 @@ class LazySeries:
     # -- pandas-ish metadata
     @property
     def dtype(self):
+        if T.is_temporal(self.expr.logical):
+            return T.numpy_dtype(self.expr.logical)
         if isinstance(self.expr, ColRef):
             lg = self.expr.logical
             try:
@@ -134,6 +140,8 @@ class LazySeries:
             return o.expr
         if isinstance(o, np.generic):
             o = o.item()
+        if isinstance(o, (T.TScalar, T.Interval, str)):
+            return o            # read against the other operand's type (expr.binop / temporal.py)
         return E.as_expr(o)
 
     def _bin(self, op, o, rev=False):
@@ -196,7 +204,10 @@ class LazySeries:
         return self._wrap(E.case(self._other(cond), self.expr, self._other(other)))
 
     def astype(self, dtype):
+        unit = T.unit_of(dtype)
         s = str(dtype).lower()
+        if unit is not None:      # CAST AS DATE (datetime64[D]) / TIMESTAMP
+            return self._wrap(T.cast_to(self.expr, "D" if unit == "D" else T.DEFAULT_UNIT))
         if s in ("boolean", "bool"):
             return self._wrap(E.cast(self.expr, U8))
         if s.startswith(("int", "uint")):
@@ -242,9 +253,7 @@ class LazyFrame:
 
     def col_type(self, name):
         e = self.exprs[name]
-        if isinstance(e, ColRef):
-            return e.dtype, e.logical
-        return e.dtype, {I64: "int64", F64: "float64", U8: "bool"}[e.dtype]
+        return e.dtype, e.logical
 
     def dtype_of(self, name):
         """numpy / pandas dtype of one column (cheap: no Series is built)."""

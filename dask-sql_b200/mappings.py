@@ -3,6 +3,7 @@ BIGINT / DOUBLE / BOOLEAN and the narrower numeric types that widen onto them)."
 import numpy as np
 import pandas as pd
 
+from . import temporal as T
 from .frame import LazyFrame, LazySeries
 
 
@@ -10,7 +11,7 @@ class SqlTypeName:
     """String-valued stand-in for the Rust enum dask_sql._datafusion_lib.SqlTypeName."""
 
     _names = ["ANY", "BIGINT", "BOOLEAN", "DOUBLE", "FLOAT", "REAL", "INTEGER", "SMALLINT", "TINYINT",
-              "DECIMAL", "NULL", "VARCHAR", "CHAR", "DATE", "TIMESTAMP", "TIME"]
+              "DECIMAL", "NULL", "VARCHAR", "CHAR", "DATE", "TIMESTAMP", "TIME", "INTERVAL"]
 
     def __init__(self, name):
         self.name = name.upper()
@@ -61,8 +62,12 @@ _SQL_TO_PYTHON = {
 
 
 def python_to_sql_type(python_type) -> SqlTypeName:
-    """mappings.py:92-116."""
+    """mappings.py:92-116.  datetime64[D] (and date32) is DATE, datetime64[s|ms|us|ns] is TIMESTAMP;
+    time-zone-aware and timedelta types are not supported."""
     key = str(python_type)
+    sql = T.sql_type_of(key)
+    if sql is not None:
+        return SqlTypeName(sql)
     try:
         return _PYTHON_TO_SQL[key]
     except KeyError:
@@ -71,6 +76,10 @@ def python_to_sql_type(python_type) -> SqlTypeName:
 
 def sql_to_python_type(sql_type, *args):
     name = sql_type.name if isinstance(sql_type, SqlTypeName) else SqlTypeName.fromString(sql_type).name
+    if name == "DATE":
+        return np.dtype("datetime64[D]")
+    if name == "TIMESTAMP":
+        return np.dtype(f"datetime64[{T.DEFAULT_UNIT}]")
     try:
         return _SQL_TO_PYTHON[name]
     except KeyError:
@@ -85,11 +94,27 @@ def sql_to_python_value(sql_type, literal_value):
     if name in ("DOUBLE", "FLOAT", "REAL", "DECIMAL"):
         return float(literal_value)
     if name in ("BIGINT", "INTEGER", "SMALLINT", "TINYINT"):
+        if isinstance(literal_value, T.TScalar):       # CAST(DATE '...' AS BIGINT): its ticks
+            return literal_value.ticks
         return int(literal_value)
     if name == "BOOLEAN":
         return bool(literal_value)
     if name in ("VARCHAR", "CHAR"):
         return str(literal_value)
+    if name in ("DATE", "TIMESTAMP"):
+        # a DATE / TIMESTAMP value, or a string read as one (CAST('1995-03-15' AS DATE))
+        if isinstance(literal_value, T.TScalar):
+            if name == "DATE":
+                return T.TScalar(T.datepart(literal_value.ticks, "DAYS", literal_value.unit), "D")
+            return T.TScalar(literal_value.at(T.DEFAULT_UNIT), T.DEFAULT_UNIT) if literal_value.unit == "D" \
+                else literal_value
+        try:
+            return T.parse_date(str(literal_value)) if name == "DATE" else T.parse_timestamp(str(literal_value))
+        except ValueError as err:
+            from .utils import ParsingException
+            raise ParsingException(str(literal_value), str(err)) from None
+    if name == "INTERVAL" and isinstance(literal_value, T.Interval):
+        return literal_value
     raise NotImplementedError(f"literal of SQL type {name}")
 
 
@@ -102,6 +127,11 @@ def similar_type(lhs, rhs) -> bool:
     hit = _SIMILAR_CACHE.get(key)
     if hit is not None:
         return hit
+    ul, ur = T.unit_of(lhs), T.unit_of(rhs)
+    if ul is not None or ur is not None:     # DATE and TIMESTAMP are two families; units do not matter
+        out = ul is not None and ur is not None and (ul == "D") == (ur == "D")
+        _SIMILAR_CACHE[key] = out
+        return out
     pdt = pd.api.types
     l, r = pd.api.types.pandas_dtype(lhs), pd.api.types.pandas_dtype(rhs)
     out = False

@@ -79,6 +79,29 @@ def _conjunction(terms):
     return series
 
 
+def _same_unit_keys(left, right, left_on, right_on):
+    """DATE / TIMESTAMP keys of different units meet at the finer one: the coarser side joins on a
+    scaled copy of its key column (the shown columns stay the inputs' own)."""
+    from .... import temporal as T
+    from ....utils import new_temporary_column
+
+    left_on, right_on = list(left_on), list(right_on)
+    for i, (a, b) in enumerate(zip(left_on, right_on)):
+        ua, ub = T.unit_of(left.col_type(a)[1]), T.unit_of(right.col_type(b)[1])
+        if ua is None or ub is None or ua == ub:
+            continue
+        u = T.finer(ua, ub)
+        if ua != u:
+            name = new_temporary_column(left)
+            left = left.assign(**{name: left[a]._wrap(T.at_unit(left[a].expr, u))})
+            left_on[i] = name
+        else:
+            name = new_temporary_column(right)
+            right = right.assign(**{name: right[b]._wrap(T.at_unit(right[b].expr, u))})
+            right_on[i] = name
+    return left, right, left_on, right_on
+
+
 class DaskJoinPlugin(BaseRelPlugin):
     class_name = "Join"
 
@@ -94,11 +117,12 @@ class DaskJoinPlugin(BaseRelPlugin):
         if not pairs:
             raise NotImplementedError(
                 "joins without an equality key (cross joins) are outside the hash-join hot path of this layer")
-        joined = left.merge(right, how=how, broadcast=dask_config.get("sql.join.broadcast"),
-                            left_on=[left.columns[i] for i, _ in pairs],
-                            right_on=[right.columns[j] for _, j in pairs])
-
         shown = list(left.columns) + ([] if how in _LEFT_ONLY_OUTPUT else list(right.columns))
+        left_on, right_on = [left.columns[i] for i, _ in pairs], [right.columns[j] for _, j in pairs]
+        left, right, left_on, right_on = _same_unit_keys(left, right, left_on, right_on)
+        joined = left.merge(right, how=how, broadcast=dask_config.get("sql.join.broadcast"),
+                            left_on=left_on, right_on=right_on)
+
         row_type = rel.getRowType()
         names = self.fix_column_to_row_type(ColumnContainer(joined.columns).limit_to(shown), row_type, how)
         out = DataContainer(joined, names)

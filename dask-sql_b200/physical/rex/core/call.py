@@ -13,6 +13,7 @@ import operator
 
 import numpy as np
 
+from .... import temporal as T
 from ....mappings import SqlTypeName, cast_column_to_type, sql_to_python_type, sql_to_python_value
 from ....utils import LoggableDataFrame, is_frame
 from ..base import BaseRexPlugin
@@ -174,6 +175,25 @@ def _in_list(args, rex):
     return (x in candidates) != bool(rex.isNegated())
 
 
+def _temporal(build, nstatic):
+    """DATE / TIMESTAMP function: the first `nstatic` operands are words (field, unit), the rest values.
+    Builds the device expression (temporal.py); on scalars the same tree is folded on the host."""
+    from .... import expr as E
+    from ....frame import LazySeries
+
+    def run(args, rex):
+        words, vals = list(args[:nstatic]), list(args[nstatic:])
+        if any(v is None for v in vals):
+            return None
+        src = next((v for v in vals if is_frame(v)), None)
+        exprs = [v.expr if is_frame(v) else (v if isinstance(v, str) else E.as_expr(v)) for v in vals]
+        e = build(*words, *exprs)
+        if src is None:
+            return T.fold(e)
+        return LazySeries(src.source, src.pred, e)
+    return run
+
+
 _COMPARISONS = {"=": operator.eq, "!=": operator.ne, "<>": operator.ne, ">": operator.gt, ">=": operator.ge,
                 "<": operator.lt, "<=": operator.le}
 
@@ -201,6 +221,16 @@ OPERATORS.update({
     "cast": _cast,
     "between": _between,
     "in list": _in_list,
+    # DATE / TIMESTAMP (the reference's names, call.py:1137-1155)
+    "date_part": _temporal(T.extract, 1),
+    "datepart": _temporal(T.extract, 1),
+    "extract_date": _temporal(lambda x: T.extract("DATE", x), 0),
+    "year": _temporal(lambda x: T.extract("YEAR", x), 0),
+    "timestampadd": _temporal(T.timestampadd, 1),
+    "timestampdiff": _temporal(T.timestampdiff, 1),
+    "timestampfloor": _temporal(lambda x, unit: T.floor_ceil(x, unit, False), 0),
+    "timestampceil": _temporal(lambda x, unit: T.floor_ceil(x, unit, True), 0),
+    "last_day": _temporal(lambda x: T.add_months_expr(x, 0, to_last=True), 0),
 })
 
 

@@ -9,6 +9,8 @@ _ARROW_TO_SQL = {
     "Int64": ("BIGINT", "getInt64Value"), "UInt8": ("TINYINT", "getUInt8Value"),
     "UInt16": ("SMALLINT", "getUInt16Value"), "UInt32": ("INTEGER", "getUInt32Value"),
     "UInt64": ("BIGINT", "getUInt64Value"), "Utf8": ("VARCHAR", "getStringValue"),
+    "Date32": ("DATE", "getTemporalValue"), "Timestamp": ("TIMESTAMP", "getTemporalValue"),
+    "IntervalMonthDayNano": ("INTERVAL", "getTemporalValue"),
 }
 
 

@@ -3,6 +3,7 @@ src/sql.rs:586-596), for the hot-path grammar.  Produces the same plan SHAPES th
 plugins expect: Projection / Aggregate / Filter / Join / SubqueryAlias / TableScan."""
 from typing import Callable, Dict, List, Optional, Tuple
 
+from .. import temporal as T
 from ..utils import ParsingException
 from . import plan as P
 from .plan import PyExpr, RelDataTypeField
@@ -11,7 +12,9 @@ from .sqlparse import Node
 _NUMERIC = ("BIGINT", "DOUBLE", "INTEGER", "FLOAT", "SMALLINT", "TINYINT", "REAL", "DECIMAL")
 _CAST_TYPES = {"BIGINT": "BIGINT", "INT": "BIGINT", "INTEGER": "BIGINT", "SMALLINT": "BIGINT", "TINYINT": "BIGINT",
                "DOUBLE": "DOUBLE", "FLOAT": "DOUBLE", "REAL": "DOUBLE", "DECIMAL": "DOUBLE", "NUMERIC": "DOUBLE",
-               "BOOLEAN": "BOOLEAN", "BOOL": "BOOLEAN", "VARCHAR": "VARCHAR", "STRING": "VARCHAR", "TEXT": "VARCHAR"}
+               "BOOLEAN": "BOOLEAN", "BOOL": "BOOLEAN", "VARCHAR": "VARCHAR", "STRING": "VARCHAR", "TEXT": "VARCHAR",
+               "DATE": "DATE", "TIMESTAMP": "TIMESTAMP"}
+_TEMPORAL = ("DATE", "TIMESTAMP")
 
 
 def _norm_type(t: str) -> str:
@@ -220,6 +223,16 @@ class Binder:
         k = e.kind
         if k == "lit":
             return P.lit(e.value)
+        if k == "typed_lit":
+            try:
+                return P.lit(T.parse_date(e.value) if e.type == "DATE" else T.parse_timestamp(e.value))
+            except ValueError as err:
+                self.err(str(err))
+        if k == "interval":
+            try:
+                return P.lit(T.parse_interval(e.value, e.unit))
+            except ValueError as err:
+                self.err(str(err))
         if k == "col":
             parts = e.parts
             if len(parts) == 1:
@@ -256,6 +269,8 @@ class Binder:
             if op in ("=", "!=", "<", "<=", ">", ">="):
                 return PyExpr("binary", "BOOLEAN", op=op, args=[l, r])
             if op in ("+", "-", "*", "/", "%"):
+                if {l.sql_type, r.sql_type} & {"DATE", "TIMESTAMP", "INTERVAL"}:
+                    return PyExpr("binary", self._temporal_arith(op, l, r), op=op, args=[l, r])
                 return PyExpr("binary", _arith_type(l.sql_type, r.sql_type), op=op, args=[l, r])
             self.err(f"Unsupported operator {op}")
         if k == "not":
@@ -303,6 +318,9 @@ class Binder:
                     self.err(f"{name} takes exactly one argument")
                 if any(a.contains_agg() for a in args):
                     self.err("Aggregate function calls cannot be nested")
+                if name not in ("COUNT", "MIN", "MAX") and any(a.sql_type in _TEMPORAL for a in args):
+                    raise NotImplementedError(f"{name} of a {args[0].sql_type}: only COUNT, MIN and MAX aggregate "
+                                              "dates and timestamps")
                 if name.startswith("BIT_") and args[0].sql_type not in ("BIGINT", "INTEGER", "SMALLINT", "TINYINT"):
                     self.err(f"{name} takes an integer argument, not {args[0].sql_type}")
                 if name == "EVERY" and args[0].sql_type != "BOOLEAN":
@@ -317,8 +335,78 @@ class Binder:
                     ty = args[0].sql_type
                 filt = rec(e.filter) if e.filter is not None else None
                 return PyExpr("agg", ty, name=name, args=args, distinct=e.distinct, filter=filt)
+            if name in _TEMPORAL_FUNCS:
+                return self._bind_temporal(name, e.args, rec)
             args = [rec(a) for a in e.args]
             if name == "ABS" and len(args) == 1:
                 return PyExpr("scalarfn", _norm_type(args[0].sql_type), name="abs", args=args)
             self.err(f"Function {name} is outside the int64/float64 hot path of this layer")
         self.err(f"Unsupported expression {k}")
+
+    # -- DATE / TIMESTAMP ---------------------------------------------------------------------
+    def _temporal_arith(self, op, l, r) -> str:
+        """DATE / TIMESTAMP +- INTERVAL keeps its type; a DATE plus a sub-day interval is a TIMESTAMP."""
+        if op in ("+", "-") and r.sql_type == "INTERVAL" and l.sql_type in _TEMPORAL + ("NULL",):
+            if l.sql_type == "DATE" and r.kind == "literal" and r.value is not None and r.value.ns % T.NS_PER_DAY:
+                return "TIMESTAMP"
+            return l.sql_type
+        if op == "+" and l.sql_type == "INTERVAL" and r.sql_type in _TEMPORAL:
+            return self._temporal_arith(op, r, l)
+        if op == "-" and l.sql_type in _TEMPORAL and r.sql_type in _TEMPORAL:
+            raise NotImplementedError("the difference of two dates / timestamps is an interval, which is not a "
+                                      "column type here; use TIMESTAMPDIFF(unit, a, b)")
+        raise NotImplementedError(f"{l.sql_type} {op} {r.sql_type}: dates and timestamps take +/- INTERVAL only")
+
+    def _unit_arg(self, node) -> str:
+        """TIMESTAMPADD(YEAR, ...): the unit is a bare word (a column node) or a string."""
+        word = node.parts[-1] if node.kind == "col" else node.value
+        try:
+            return T.norm_unit(word)
+        except ValueError as err:
+            self.err(str(err))
+
+    def _temporal_arg(self, name, x):
+        if x.sql_type not in _TEMPORAL + ("NULL",):
+            self.err(f"{name} takes a DATE or TIMESTAMP argument, not {x.sql_type}")
+        return x
+
+    def _bind_temporal(self, name, nodes, rec) -> PyExpr:
+        """EXTRACT / DATE_PART / YEAR / TIMESTAMPADD / TIMESTAMPDIFF / FLOOR, CEIL(x TO u) / LAST_DAY, under
+        the operator names of the reference's table (call.py:1137-1155)."""
+        want = {"EXTRACT": 2, "DATE_PART": 2, "DATEPART": 2, "YEAR": 1, "TIMESTAMPADD": 3, "TIMESTAMPDIFF": 3,
+                "TIMESTAMPFLOOR": 2, "TIMESTAMPCEIL": 2, "LAST_DAY": 1}[name]
+        if len(nodes) != want:
+            self.err(f"{name} takes {want} argument(s)")
+        if name in ("EXTRACT", "DATE_PART", "DATEPART"):
+            try:
+                field = T.extract_field(nodes[0].value)
+            except NotImplementedError:
+                self.err(f"EXTRACT: unknown field {nodes[0].value}")
+            x = self._temporal_arg(name, rec(nodes[1]))
+            return PyExpr("scalarfn", "DATE" if field == "DATE" else "BIGINT", name="date_part",
+                          args=[P.lit(field), x])
+        if name == "YEAR":
+            return PyExpr("scalarfn", "BIGINT", name="year", args=[self._temporal_arg(name, rec(nodes[0]))])
+        if name == "LAST_DAY":
+            x = self._temporal_arg(name, rec(nodes[0]))
+            return PyExpr("scalarfn", x.sql_type, name="last_day", args=[x])
+        if name in ("TIMESTAMPFLOOR", "TIMESTAMPCEIL"):
+            x = self._temporal_arg(name, rec(nodes[0]))
+            return PyExpr("scalarfn", x.sql_type, name=name.lower(), args=[x, P.lit(self._unit_arg(nodes[1]))])
+        unit = self._unit_arg(nodes[0])
+        if name == "TIMESTAMPADD":
+            n, x = rec(nodes[1]), self._temporal_arg(name, rec(nodes[2]))
+            if n.sql_type not in ("BIGINT", "INTEGER", "SMALLINT", "TINYINT", "NULL"):
+                self.err(f"TIMESTAMPADD takes an integer amount, not {n.sql_type}")
+            ty = x.sql_type
+            if ty == "DATE" and unit not in ("YEAR", "QUARTER", "MONTH", "WEEK", "DAY"):
+                ty = "TIMESTAMP"
+            return PyExpr("scalarfn", ty, name="timestampadd", args=[P.lit(unit), n, x])
+        a, b = rec(nodes[1]), rec(nodes[2])
+        if a.sql_type not in _TEMPORAL and b.sql_type not in _TEMPORAL:
+            self.err("TIMESTAMPDIFF takes DATE or TIMESTAMP arguments")
+        return PyExpr("scalarfn", "BIGINT", name="timestampdiff", args=[P.lit(unit), a, b])
+
+
+_TEMPORAL_FUNCS = ("EXTRACT", "DATE_PART", "DATEPART", "YEAR", "TIMESTAMPADD", "TIMESTAMPDIFF", "TIMESTAMPFLOOR",
+                   "TIMESTAMPCEIL", "LAST_DAY")

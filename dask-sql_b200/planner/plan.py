@@ -6,6 +6,7 @@ importable its plans can be fed to the same plugins because they only rely on th
 """
 from typing import List, Optional, Sequence, Tuple
 
+from .. import temporal as T
 from ..mappings import SqlTypeName
 
 
@@ -90,7 +91,8 @@ for _n in ("Reference", "Call", "Literal", "Alias", "ScalarSubquery"):
 # expressions
 # ---------------------------------------------------------------------------------------------
 _ARROW = {"BIGINT": "Int64", "DOUBLE": "Float64", "BOOLEAN": "Boolean", "VARCHAR": "Utf8", "NULL": "Null",
-          "INTEGER": "Int32", "FLOAT": "Float32"}
+          "INTEGER": "Int32", "FLOAT": "Float32", "DATE": "Date32", "TIMESTAMP": "Timestamp",
+          "INTERVAL": "IntervalMonthDayNano"}
 AGG_FUNCS = {"SUM", "AVG", "COUNT", "MIN", "MAX", "MEAN", "STDDEV", "STDDEV_SAMP", "STDDEV_POP", "VAR_SAMP",
              "VAR_POP", "VARIANCE", "BIT_AND", "BIT_OR", "BIT_XOR", "EVERY", "REGR_COUNT", "REGR_SXX", "REGR_SYY"}
 
@@ -156,6 +158,8 @@ class PyExpr:
                 return f"Int64({self.value})"
             if isinstance(self.value, float):
                 return f"Float64({self.value!r})"
+            if self.sql_type in ("DATE", "TIMESTAMP", "INTERVAL"):
+                return f'{_ARROW[self.sql_type]}("{self.value}")'
             return f'Utf8("{self.value}")'
         if k == "binary":
             return f"{self.args[0].display()} {self.op} {self.args[1].display()}"
@@ -308,6 +312,10 @@ class PyExpr:
     def getStringValue(self):
         return str(self.value)
 
+    def getTemporalValue(self):
+        """DATE / TIMESTAMP literal: a temporal.TScalar; INTERVAL: a temporal.Interval"""
+        return self.value
+
 
 def col(qualifier, name, sql_type):
     return PyExpr("column", sql_type, qualifier=qualifier, name=name)
@@ -322,6 +330,10 @@ def lit(value):
         return PyExpr("literal", "BIGINT", value=value)
     if isinstance(value, float):
         return PyExpr("literal", "DOUBLE", value=value)
+    if isinstance(value, T.TScalar):
+        return PyExpr("literal", T.sql_type_of(value.logical), value=value)
+    if isinstance(value, T.Interval):
+        return PyExpr("literal", "INTERVAL", value=value)
     return PyExpr("literal", "VARCHAR", value=value)
 
 

@@ -10,8 +10,9 @@ that crate cannot be built here (no rustc/cargo), so this is a small recursive-d
   source := table [[AS] alias] | ( select ) [AS] alias
   join   := [INNER | LEFT [OUTER] | RIGHT [OUTER] | FULL [OUTER] | CROSS] JOIN source [ON e]
 
-Expressions: literals, [qualifier.]column, + - * / %, comparisons, AND OR NOT, IS [NOT] NULL,
-[NOT] BETWEEN, [NOT] IN (list), CAST(e AS type), CASE WHEN, function calls incl. aggregates with
+Expressions: literals (incl. DATE '...', TIMESTAMP '...', INTERVAL '...' [unit]), [qualifier.]column,
++ - * / %, comparisons, AND OR NOT, IS [NOT] NULL, [NOT] BETWEEN, [NOT] IN (list), CAST(e AS type),
+CASE WHEN, EXTRACT(field FROM e), FLOOR / CEIL(e TO unit), function calls incl. aggregates with
 DISTINCT and FILTER (WHERE ...).
 
 Statements around the path (custom statements of the reference's parser, src/parser.rs):
@@ -38,6 +39,10 @@ KEYWORDS = {"SELECT", "FROM", "WHERE", "GROUP", "BY", "HAVING", "ORDER", "LIMIT"
             "NOT", "IS", "NULL", "IN", "BETWEEN", "JOIN", "INNER", "LEFT", "RIGHT", "FULL", "OUTER", "CROSS", "ON",
             "DISTINCT", "CASE", "WHEN", "THEN", "ELSE", "END", "CAST", "TRUE", "FALSE", "ASC", "DESC", "NULLS",
             "FIRST", "LAST", "WITH", "FILTER", "UNION", "ALL", "EXPLAIN", "SEMI", "ANTI", "USING"}
+
+
+_TIME_UNITS = {"YEAR", "QUARTER", "MONTH", "WEEK", "DAY", "HOUR", "MINUTE", "SECOND", "MILLISECOND", "MICROSECOND",
+               "NANOSECOND"}
 
 
 class Tok:
@@ -487,6 +492,23 @@ class Parser:
             other = self.parse_expr() if self.eat_kw("ELSE") else None
             self.expect_kw("END")
             return Node("case", whens=whens, other=other)
+        nxt = self.toks[self.i + 1] if self.i + 1 < len(self.toks) else t
+        if t.kind == "id" and t.val.upper() in ("DATE", "TIMESTAMP") and nxt.kind == "str":
+            self.i += 2                                   # DATE 'YYYY-MM-DD', TIMESTAMP 'YYYY-MM-DD HH:MM:SS'
+            return Node("typed_lit", type=t.val.upper(), value=nxt.val)
+        if t.kind == "id" and t.val.upper() == "INTERVAL" and nxt.kind == "str":
+            self.i += 2                                   # INTERVAL '4 days' | INTERVAL '4' DAY
+            unit = self.ident().upper() if self.cur.kind == "id" and self.cur.val.upper().rstrip("S") in _TIME_UNITS \
+                else None
+            return Node("interval", value=nxt.val, unit=unit)
+        if t.kind == "id" and t.val.upper() == "EXTRACT" and nxt.kind == "op" and nxt.val == "(":
+            self.i += 2                                   # EXTRACT(field FROM x)
+            field = self.ident().upper()
+            self.expect_kw("FROM")
+            x = self.parse_expr()
+            self.expect_op(")")
+            return Node("func", name="EXTRACT", args=[Node("lit", value=field), x], distinct=False, star=False,
+                        filter=None)
         if t.kind == "id" or (t.kind == "kw" and t.val in ("LEFT", "RIGHT", "FIRST", "LAST", "FILTER")
                               and self.toks[self.i + 1].kind == "op" and self.toks[self.i + 1].val in ("(", ".")):
             name = self.ident() if t.kind == "id" else (self.toks[self.i].val, setattr(self, "i", self.i + 1))[0]
@@ -497,6 +519,11 @@ class Parser:
                     star = True
                 elif not self.at_op(")"):
                     args.append(self.parse_expr())
+                    if name.upper() in ("FLOOR", "CEIL") and self.eat_word("TO"):   # FLOOR(x TO unit)
+                        args.append(Node("lit", value=self.ident().upper()))
+                        self.expect_op(")")
+                        return Node("func", name="TIMESTAMP" + name.upper(), args=args, distinct=False,
+                                    star=False, filter=None)
                     while self.eat_op(","):
                         args.append(self.parse_expr())
                 self.expect_op(")")

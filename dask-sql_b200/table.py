@@ -12,6 +12,7 @@ from typing import Dict, List, Optional
 import numpy as np
 import torch
 
+from . import temporal as T
 from .device import DeviceColumn, Stats, column_from_host, I64, F64, U8, _pack_valid
 
 
@@ -77,7 +78,10 @@ def _arrow_array_to_column(arr) -> ArrowColumn:
 
     t = arr.type
     n = len(arr)
-    if pa.types.is_dictionary(t) or pa.types.is_string(t) or pa.types.is_large_string(t) or pa.types.is_temporal(t) \
+    # DATE: date32 (days) / date64 (ms -> days); TIMESTAMP: timestamp[unit] without a time zone
+    date_or_ts = pa.types.is_date(t) or (pa.types.is_timestamp(t) and t.tz is None)
+    if pa.types.is_dictionary(t) or pa.types.is_string(t) or pa.types.is_large_string(t) \
+            or (pa.types.is_temporal(t) and not date_or_ts) \
             or pa.types.is_decimal(t) or pa.types.is_nested(t) or pa.types.is_uint64(t):
         raise NotImplementedError(
             f"column type {t} is outside the int64/float64/bool hot path of this layer")
@@ -92,6 +96,14 @@ def _arrow_array_to_column(arr) -> ArrowColumn:
         else:   # a slice that does not start on a byte boundary: realign once
             bits = np.unpackbits(vb, bitorder="little")[off: off + n]
             valid_bytes = np.packbits(bits, bitorder="little")
+    if date_or_ts:
+        if pa.types.is_date32(t):
+            vals, unit = np.frombuffer(bufs[1], dtype=np.int32)[off: off + n].astype(np.int64), "D"
+        elif pa.types.is_date64(t):
+            vals, unit = np.frombuffer(bufs[1], dtype=np.int64)[off: off + n] // 86_400_000, "D"
+        else:
+            vals, unit = np.frombuffer(bufs[1], dtype=np.int64)[off: off + n], t.unit
+        return ArrowColumn(vals, valid_bytes, T.logical_of(unit))
     if pa.types.is_boolean(t):
         bits = np.unpackbits(np.frombuffer(bufs[1], dtype=np.uint8), bitorder="little")[off: off + n]
         return ArrowColumn(np.ascontiguousarray(bits, dtype=np.uint8).view(np.bool_), valid_bytes,
@@ -178,6 +190,8 @@ def _host_column(values, pin=True) -> HostColumn:
         vals = values
     else:
         vals = np.asarray(values)
+    if not isinstance(vals, torch.Tensor) and vals.dtype.kind == "M":
+        vals, mask, logical = T.from_host_array(vals)      # DATE / TIMESTAMP ticks, NaT -> NULL
     if isinstance(vals, torch.Tensor):
         t = vals
         dt = {torch.int64: I64, torch.float64: F64, torch.uint8: U8, torch.bool: U8}[t.dtype]
@@ -188,6 +202,8 @@ def _host_column(values, pin=True) -> HostColumn:
         kind = vals.dtype.kind
         if kind == "b":
             vals, dt = vals.astype(np.uint8), U8
+        elif T.is_temporal(logical):
+            dt = I64
         elif kind in "iu" and not (kind == "u" and vals.dtype.itemsize == 8):
             vals, dt = vals.astype(np.int64, copy=False), I64
         elif kind == "f":
@@ -346,6 +362,13 @@ class ParquetTable(DeviceTable):
         names = [self.file.schema_arrow.names[i] for i in range(len(self.file.schema_arrow.names))]
         self._names = [n for n in names if columns is None or n in columns]
         self._nrows = md.num_rows
+        import pyarrow as pa
+        units = {}
+        for f in self.file.schema_arrow:
+            if pa.types.is_date(f.type):
+                units[f.name] = "D"
+            elif pa.types.is_timestamp(f.type) and f.type.tz is None:
+                units[f.name] = f.type.unit
         self._groups = []                       # per row group: {"rows": n, "cols": {name: {"min","max","nulls","rows"} | None}}
         for g in range(md.num_row_groups):
             rg = md.row_group(g)
@@ -355,7 +378,11 @@ class ParquetTable(DeviceTable):
                 st = col.statistics
                 nm = col.path_in_schema
                 if st is not None and st.has_min_max and st.has_null_count:
-                    cols[nm] = {"min": st.min, "max": st.max, "nulls": st.null_count, "rows": rg.num_rows}
+                    lo, hi = st.min, st.max
+                    unit = units.get(nm)
+                    if unit is not None:       # datetime.date / datetime statistics -> ticks of the column's unit
+                        lo, hi = T.stat_to_ticks(lo, unit), T.stat_to_ticks(hi, unit)
+                    cols[nm] = {"min": lo, "max": hi, "nulls": st.null_count, "rows": rg.num_rows}
                 else:
                     cols[nm] = None
             self._groups.append({"rows": rg.num_rows, "cols": cols})

@@ -175,6 +175,26 @@ typedef struct b2_prog {
 #define B2_OP_CASE     55   /* pops else, then, cond: cond true -> then, else (or NULL cond) -> else */
 #define B2_OP_FILLNA   56   /* pops fill, x: x if valid else fill */
 #define B2_OP_ORD2F    57   /* order-preserving int64 image -> float64 (float MIN/MAX accumulators) */
+/* Calendar opcodes on DATE / TIMESTAMP ticks.  imm_i = ticks per second of the operand's unit
+ * (1, 10^3, 10^6, 10^9), or 0 when the operand counts days since 1970-01-01.  The split into
+ * (day, time of day) is floored, so -1 us is 1969-12-31 23:59:59.999999. */
+#define B2_OP_DATEPART  60  /* pops x, pushes field a of x (B2_DP_*) */
+#define B2_OP_ADDMONTHS 61  /* pops n, x: x moved by n calendar months, day clamped to the month's end,
+                               time of day kept; a = 1: then moved to the last day of its month */
+#define B2_DP_DAYS         0   /* floor to days since the epoch (CAST AS DATE) */
+#define B2_DP_YEAR         1
+#define B2_DP_QUARTER      2
+#define B2_DP_MONTH        3
+#define B2_DP_DAY          4
+#define B2_DP_DOY          5   /* 1..366 */
+#define B2_DP_DOW          6   /* 0 = Sunday .. 6 = Saturday */
+#define B2_DP_ISOWEEK      7   /* ISO 8601 week 1..53 */
+#define B2_DP_HOUR         8
+#define B2_DP_MINUTE       9
+#define B2_DP_SECOND      10
+#define B2_DP_MILLISECOND 11   /* within the second, 0..999 */
+#define B2_DP_MICROSECOND 12   /* within the second, 0..999999 */
+#define B2_DP_NFIELDS     13
 
 /* ---- runtime --------------------------------------------------------------------- */
 const char* b2_last_error(void);
