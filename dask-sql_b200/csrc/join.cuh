@@ -848,14 +848,23 @@ static int32_t b2_check_join(const b2_scan_t* scan, const int32_t* probe_keys, c
   B2_REQUIRE(probe_keys && jt, "null argument");
   B2_REQUIRE(jt->nkeys >= 1 && jt->nkeys <= B2_MAX_KEYS, "bad nkeys");
   B2_REQUIRE(mode >= B2_JOIN_INNER && mode <= B2_JOIN_ANTI, "bad join mode");
+  B2_REQUIRE(jt->dense >= 0 && jt->dense <= 2, "bad table kind");
   memset(pk, 0, sizeof(*pk));
   for (int k = 0; k < jt->nkeys; ++k) {
+    // b2_for_matches loads build keys as 8-byte words: a one-byte key column would be read past its end
+    B2_REQUIRE(jt->keys[k].dtype == B2_I64 || jt->keys[k].dtype == B2_F64, "join keys must be int64 or float64");
     B2_REQUIRE(probe_keys[k] >= 0 && probe_keys[k] < scan->ncols, "probe key out of range");
     B2_REQUIRE(scan->cols[probe_keys[k]].dtype == jt->keys[k].dtype, "probe/build key types differ");
     pk->cols[k] = probe_keys[k];
   }
-  if (jt->dense) B2_REQUIRE(jt->nkeys == 1 && jt->lookup && jt->range > 0, "bad dense table");
-  else B2_REQUIRE(jt->head && b2_pow2(jt->cap), "bad chained table");
+  if (jt->dense) {
+    B2_REQUIRE(jt->nkeys == 1 && jt->lookup && jt->range > 0, "bad dense table");
+    B2_REQUIRE(jt->keys[0].dtype == B2_I64, "a direct-address table needs an int64 key");
+    // a key-ordered table's build row is the key offset, held in an int32
+    B2_REQUIRE(jt->dense == 1 || jt->range < (1LL << 31), "key-ordered table needs range < 2^31");
+  } else {
+    B2_REQUIRE(jt->head && b2_pow2(jt->cap), "bad chained table");
+  }
   return B2_OK;
 }
 
@@ -882,11 +891,13 @@ int32_t b2_join_count(const b2_scan_t* scan, const int32_t* probe_keys, const b2
   return B2_OK;
 }
 
-static int32_t b2_fill_joingather(const b2_scan_t* scan, const b2_jointable_t* jt, int32_t nprobe,
+static int32_t b2_fill_joingather(const b2_scan_t* scan, const b2_jointable_t* jt, int32_t mode, int32_t nprobe,
                                   const int32_t* probe_cols, void* const* probe_out, uint32_t* const* probe_valid,
                                   int32_t nbuild, const b2_col_t* build_cols, const int64_t* build_base,
                                   void* const* build_out, uint32_t* const* build_valid, b2_joingather_arg* g) {
   B2_REQUIRE(nprobe >= 0 && nprobe <= B2_MAX_GATHER && nbuild >= 0 && nbuild <= B2_MAX_GATHER, "too many gather columns");
+  // a SEMI / ANTI row has no build row: the chained and direct-address kernels would fill such columns differently
+  B2_REQUIRE(nbuild == 0 || mode == B2_JOIN_INNER || mode == B2_JOIN_LEFT, "build columns need an INNER or LEFT join");
   memset(g, 0, sizeof(*g));
   g->nprobe = nprobe;
   g->nbuild = nbuild;
@@ -918,8 +929,10 @@ int32_t b2_join_write_gather_keyed(const b2_scan_t* scan, const int32_t* probe_k
   int32_t rc = b2_check_join(scan, probe_keys, jt, mode, &pk);
   if (rc) return rc;
   B2_REQUIRE(d_tile_off, "null argument");
+  // the chained SEMI probe stops at the first partner; ANTI rows have none
+  B2_REQUIRE(!build_matched || mode == B2_JOIN_INNER || mode == B2_JOIN_LEFT, "build_matched needs an INNER or LEFT join");
   b2_joingather_arg g;
-  rc = b2_fill_joingather(scan, jt, nprobe, probe_cols, probe_out, probe_valid, nbuild, build_cols, build_base,
+  rc = b2_fill_joingather(scan, jt, mode, nprobe, probe_cols, probe_out, probe_valid, nbuild, build_cols, build_base,
                           build_out, build_valid, &g);
   if (rc) return rc;
   const int64_t ntiles = b2_num_tiles(scan->n);
@@ -954,7 +967,7 @@ int32_t b2_join_onepass(const b2_scan_t* scan, const int32_t* probe_keys, const 
   B2_REQUIRE(d_ws, "null argument");
   B2_REQUIRE(jt->dense, "single-pass probe needs a direct-address table");
   b2_joingather_arg g;
-  rc = b2_fill_joingather(scan, jt, nprobe, probe_cols, probe_out, probe_valid, nbuild, build_cols, build_base,
+  rc = b2_fill_joingather(scan, jt, mode, nprobe, probe_cols, probe_out, probe_valid, nbuild, build_cols, build_base,
                           build_out, build_valid, &g);
   if (rc) return rc;
   const int64_t ntiles = (scan->n + B2_JOP_TILE - 1) / B2_JOP_TILE;
@@ -978,7 +991,7 @@ int32_t b2_join_onepass(const b2_scan_t* scan, const int32_t* probe_keys, const 
       else fits = false;
     }
     if (fits && nbuild == 1)
-      fits = !g.build_valid[0] && !g.build_cols[0].valid && g.build_cols[0].dtype != B2_U8 && mode == B2_JOIN_INNER;
+      fits = !g.build_valid[0] && !g.build_cols[0].valid && g.build_cols[0].dtype != B2_U8;
     if (fits) {
       const bool hp = p_col >= 0, hb = nbuild == 1, ok = key_out >= 0;
       int bmode = 0;

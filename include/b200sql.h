@@ -72,7 +72,8 @@ extern "C" {
 /* join flags */
 #define B2_JOIN_INNER        0
 #define B2_JOIN_LEFT         1   /* also emit unmatched probe rows with build index -1 */
-#define B2_JOIN_SEMI         2   /* emit each probe row once if it has >= 1 match (build index = -1) */
+#define B2_JOIN_SEMI         2   /* emit each probe row once if it has >= 1 match (build index = -1;
+                                  * no build columns, no build_matched) */
 #define B2_JOIN_ANTI         3   /* emit each probe row once if it has no match */
 
 /* empty-slot sentinel of int64 hash tables (b2_groupby_hash1, b2_star_build_hash) */
@@ -388,8 +389,12 @@ typedef struct b2_jointable {
 /* Probe with the rows of `scan` that pass its terms; probe_keys index scan.cols.
  * Same two-pass protocol as b2_select_*: count fills d_tile_off (int64[ntiles+1], exclusive
  * scan, total last), write emits (probe row, build row) pairs in probe-row order.
- * mode = B2_JOIN_*.  build_matched (uint8[n_build], may be NULL) is set to 1 for every build
- * row that found a partner (RIGHT / FULL joins, join.py:41-48). */
+ * mode = B2_JOIN_*.  build_matched (uint8[n_build], zeroed by the caller, may be NULL) is set to 1
+ * for every build row that found a partner (RIGHT / FULL joins, join.py:41-48); INNER / LEFT only:
+ * with SEMI / ANTI it must be NULL (B2_ERR_ARG otherwise).
+ * The table's keys are B2_I64 or B2_F64; a direct-address table (dense 1 or 2) has one B2_I64 key,
+ * and a key-ordered one (dense 2) a range < 2^31.  Build rows of one probe row are emitted as one
+ * contiguous run in an unspecified order. */
 int32_t b2_join_count(const b2_scan_t* scan, const int32_t* probe_keys, const b2_jointable_t* jt,
                       int32_t mode, int64_t* d_tile_off, void* stream);
 int32_t b2_join_write(const b2_scan_t* scan, const int32_t* probe_keys, const b2_jointable_t* jt,
@@ -399,8 +404,9 @@ int32_t b2_join_write(const b2_scan_t* scan, const int32_t* probe_keys, const b2
 /* b2_join_write that also gathers output columns in the same pass (the take() on every column of
  * both sides that ends pandas.merge, join.py:241-246): for each emitted pair, probe columns
  * scan.cols[probe_cols[k]] are copied to probe_out[k] and build-side columns build_cols[k] (indexed
- * by the build row, NULL for an unmatched LEFT row) to build_out[k].  *_valid[k]: validity words of
- * the output (zero-initialised by the caller, bits are OR-ed in) or NULL.  out_probe_idx /
+ * by the build row, NULL for an unmatched LEFT row) to build_out[k].  Build columns are for INNER /
+ * LEFT joins only: with SEMI / ANTI nbuild must be 0 (B2_ERR_ARG otherwise).  *_valid[k]: validity
+ * words of the output (zero-initialised by the caller, bits are OR-ed in) or NULL.  out_probe_idx /
  * out_build_idx may be NULL when the caller only wants the gathered columns. */
 int32_t b2_join_write_gather(const b2_scan_t* scan, const int32_t* probe_keys, const b2_jointable_t* jt,
                              int32_t mode, const int64_t* d_tile_off, int32_t* out_probe_idx,
