@@ -420,9 +420,13 @@ class GroupTable:
 
         new: optional allocator `new(n, torch dtype, fill value) -> tensor` for the arrays (a prepared
         multi-GPU query places them in symmetric memory so that peers can read them over NVLink)."""
-        if new is None:
-            def new(n, dtype, fill):
-                return torch.full((n,), fill, dtype=dtype, device=device)
+        self.fills = []      # (array, initial value) of every array: what reset() restores
+
+        def make(n, dtype, fill):
+            t = torch.full((n,), fill, dtype=dtype, device=device) if new is None else new(n, dtype, fill)
+            self.fills.append((t, fill))
+            return t
+
         self.device, self.nslots = device, nslots
         self.alloc = alloc = max(int(alloc or nslots), nslots)
         self.indicator = indicator
@@ -435,20 +439,26 @@ class GroupTable:
             acc = cnt = None
             if col >= 0 and op != L.AGG_COUNT:
                 if op == L.AGG_SUMF or (op == L.AGG_SUM and dt == F64):
-                    acc = new(alloc, torch.float64, -0.0 if a == indicator else 0.0)
+                    acc = make(alloc, torch.float64, -0.0 if a == indicator else 0.0)
                 else:
-                    acc = new(alloc, torch.int64, L.agg_identity(op))
+                    acc = make(alloc, torch.int64, L.agg_identity(op))
             if col >= 0 and (op == L.AGG_COUNT or need_cnt[a]):
-                cnt = new(alloc, torch.int64, 0)
+                cnt = make(alloc, torch.int64, 0)
             self.acc.append(acc)
             self.cnt.append(cnt)
             self.state.acc[a] = acc.data_ptr() if acc is not None else 0
             self.state.cnt[a] = cnt.data_ptr() if cnt is not None else 0
-        self.rows = new(alloc, torch.int64, 0) if need_rows else None
+        self.rows = make(alloc, torch.int64, 0) if need_rows else None
         need_present = need_present and indicator is None
-        self.present = new(bitmap_words(alloc), torch.int32, 0) if need_present else None
+        self.present = make(bitmap_words(alloc), torch.int32, 0) if need_present else None
         self.state.rows = self.rows.data_ptr() if self.rows is not None else 0
         self.state.present = self.present.data_ptr() if self.present is not None else 0
+
+    def reset(self):
+        """Every array back to its initial value (an empty table), in stream order: a table reused run
+        after run is refilled, not re-allocated."""
+        for t, fill in self.fills:
+            t.fill_(fill)
 
 
 def groupby_dense(scan, key_col, kmin, table: GroupTable, skew=None, hot=None):

@@ -14,6 +14,7 @@ libb200sql.so; host code only plans, allocates and moves metadata.
 """
 import ctypes as C
 import os
+from collections import namedtuple
 from typing import Dict, List, Optional, Sequence, Set
 
 import numpy as np
@@ -821,10 +822,9 @@ def _moment_shifts(aggs, parts, child, sharded):
 def run_aggregate(src: AggSource, allow_fast=True) -> Part:
     if allow_fast:
         # a fused star query that was prepared before: straight to its cached launch descriptors
-        last = src.__dict__.get("_prepared_last")
-        if last is not None and last[0] == (P.world()[1], _dev().index) and last[1] in PreparedStar._live \
-                and os.environ.get("B200SQL_NO_PREPARED") != "1":
-            return last[1].run(src)
+        cache, key = PreparedStar.cache(src)
+        if cache.get(key) is not None and os.environ.get("B200SQL_NO_PREPARED") != "1":
+            return cache[key].run(src)
     child = src.child
     pred, never = simplify_pred(child.pred)
     gexprs = [child.exprs[g] for g in src.group_cols]
@@ -1614,12 +1614,21 @@ def _side_of(e: Expr, left_names: Set[str], right_names: Set[str]):
     return "both"
 
 
+# What the shape checks of _star_dense_fast found: the join keys, the group key over the dim table's columns
+# (ge) and as the join's output names it (gexpr0, logical type glog), the aggregate plan, each side's
+# predicates and the columns it reads, the key ranges, the dim's row count (dn), and whether this rank builds
+# the lookup (owner), broadcasts it (bcast: a 'root' dim) and merges its group table with the other ranks'.
+_DenseStar = namedtuple("_DenseStar", "fk_e pk_e ge gexpr0 glog plan dpred fpred dcols fcols pmin prange gmin grng "
+                                      "gnull dn owner bcast sharded")
+
+
 class PreparedStar:
-    """Everything about one fused star query that does not change between executions, kept with the
-    (immutable) plan: launch descriptors of every dim / fact partition (ctypes structs over resident
-    columns), the aggregate plan, the lookup buffers and the group table (re-initialised, not
-    re-allocated, per run).  A step of a repeated query then costs the host a few dozen calls instead
-    of re-deriving all of it -- at 8 GPUs a step is a few ms of device work, so host time counts.
+    """The dense star pipeline of one fused star query: launch descriptors of every dim / fact partition
+    (ctypes structs over their columns), the aggregate plan, the lookup buffer and the group table.
+    Over resident table columns it is prepared once and kept with the (immutable) plan node (get()), the
+    group table re-initialised, not re-allocated, per run: a step of a repeated query then costs the host
+    a few dozen calls instead of re-deriving all of it -- at 8 GPUs a step is a few ms of device work, so
+    host time counts.  Any other query builds one over what materialize() returns and runs it once.
 
     One stream, in order: lookup build (_star_bitmap_build, on every rank that holds dim rows; a 'root'
     table is followed by one NCCL broadcast of the finished lookup) -> b2_star_agg per fact partition -> merge ->
@@ -1632,18 +1641,24 @@ class PreparedStar:
     MAX_LIVE = 4          # prepared plans keep ~100 MB of HBM each: keep only the most recent ones
 
     @classmethod
-    def get(cls, src, fact, dim, fk_e, pk_e, ge, gexpr0, aggs, fpred, dpred, meta, owner, bcast, sharded, dev):
-        key = (sharded, P.world()[1], _dev().index)
+    def cache(cls, src):
+        """(plans of `src`, this process's key): the key is (world size, device index), an entry the plan
+        or None for 'tried, not preparable'.  A plan evicted from _live (its buffers are gone) is dropped."""
         cache = src.__dict__.setdefault("_prepared_star", {})
+        key = (P.world()[1], _dev().index)
+        if cache.get(key) is not None and cache[key] not in cls._live:
+            del cache[key]
+        return cache, key
+
+    @classmethod
+    def get(cls, src, q: _DenseStar, dim, fact, dev):
+        """The cached plan of `src`, prepared on first use; None when the query's inputs do not allow one."""
+        cache, key = cls.cache(src)
         if key in cache:
-            prep = cache[key]
-            if prep is not None and prep not in cls._live:      # evicted meanwhile: its buffers are gone
-                prep = None
-                cache.pop(key)
-            else:
-                return prep
+            return cache[key]
         try:
-            prep = cls(src, fact, dim, fk_e, pk_e, ge, gexpr0, aggs, fpred, dpred, meta, owner, bcast, sharded, dev)
+            dparts = cls._resident_parts(dim.source.table, q.dcols) if q.owner else []
+            prep = cls(q, dparts, cls._resident_parts(fact.source.table, q.fcols), dev, cached=True)
         except _NotPreparable:
             prep = None
         if P.world()[1] > 1:
@@ -1652,7 +1667,7 @@ class PreparedStar:
             if int(P.allreduce_(ok, "min").item()) == 0:
                 prep = None
             else:
-                if sharded and P.peer_memory_available():
+                if q.sharded and P.peer_memory_available():
                     # collective (symmetric allocation + handle exchange): entered by all ranks or by none.
                     # A rank on which it fails (no peer access, mapping refused) says so and ALL ranks stay
                     # on the NCCL merge.
@@ -1669,88 +1684,64 @@ class PreparedStar:
                         warnings.warn(f"NVLink peer merge unavailable, using ncclReduceScatter: {why}")
         cache[key] = prep
         if prep is not None:
-            src.__dict__["_prepared_last"] = ((P.world()[1], _dev().index), prep)
             cls._live.append(prep)
             while len(cls._live) > cls.MAX_LIVE:
                 cls._live.pop(0)
         return prep
 
-    def __init__(self, src, fact, dim, fk_e, pk_e, ge, gexpr0, aggs, fpred, dpred, meta, owner, bcast, sharded, dev):
-        self.dev, self.owner, self.bcast, self.sharded = dev, owner, bcast, sharded
-        self.pmin, self.prange, self.gmin, self.grng, self.gnull, dn = meta
-        self.nslots = self.grng + 1
-        self.gname = src.group_cols[0]
-        self.gexpr0 = gexpr0
-        self.glog = dim.col_type(gexpr0.name)[1] if isinstance(gexpr0, ColRef) else "int64"
-        self.plan = AggPlan([(E.substitute(e, fact.exprs) if e is not None else None, o, f) for e, o, f in aggs],
-                            _nullable_fn(fact, sharded))
-        if any(not isinstance(ka.expr, ColRef) for ka in self.plan.kaggs):
+    def __init__(self, q: _DenseStar, dparts: List[Part], fparts: List[Part], dev, cached=False):
+        """dparts (empty unless q.owner) / fparts: the dim / fact partitions with columns q.dcols / q.fcols.
+        cached: the plan is kept and run again, so every column it reads must be a table column used as it
+        is (_NotPreparable otherwise); a plan run once evaluates computed inputs and mask predicates here."""
+        if cached and any(not isinstance(ka.expr, ColRef) for ka in q.plan.kaggs):
             raise _NotPreparable()
-        # ---- launch descriptors (every referenced column must be resident and used as it is)
+        self.q, self.dev, self.cached = q, dev, cached
+        self.nslots = q.grng + 1
+        # ---- launch descriptors; the ScanCtx objects keep the columns their scans point into alive
         self.keep = []
         self.dim_launch = []
-        if owner:
-            needed = {pk_e.name, ge.name}
-            for p in dpred:
-                p.refs(needed)
-            for part in self._resident_parts(dim.source.table, needed):
-                ctx = ScanCtx(part, dpred)
-                pk_slot, g_slot = ctx.slot(pk_e), ctx.slot(ge)
-                self._only_table_columns(ctx)
-                self.dim_launch.append((ctx.scan(), pk_slot, g_slot))
-                self.keep.append(ctx)
-        needed = set(fk_e.refs())
-        for ka in self.plan.kaggs:
-            ka.expr.refs(needed)
-        for p in fpred:
-            p.refs(needed)
+        for part in dparts:
+            if part.n == 0:
+                continue
+            ctx = ScanCtx(part, q.dpred)
+            pk_slot, g_slot = ctx.slot(q.pk_e), ctx.slot(q.ge)     # slots first: scan() snapshots the columns
+            self._only_table_columns(ctx)
+            self.dim_launch.append((ctx.scan(), pk_slot, g_slot))
+            self.keep.append(ctx)
         self.fact_launch = []
-        for part in self._resident_parts(fact.source.table, needed):
-            ctx = ScanCtx(part, fpred)
-            fk_slot = ctx.slot(fk_e)
-            specs = [(ctx.slot(ka.expr), ka.op) for ka in self.plan.kaggs]
+        for part in fparts:
+            if part.n == 0:
+                continue
+            ctx = ScanCtx(part, q.fpred)
+            fk_slot = ctx.slot(q.fk_e)
+            specs = [(ctx.slot(ka.expr), ka.op) for ka in q.plan.kaggs]
             self._only_table_columns(ctx)
             self.fact_launch.append((ctx.scan(), fk_slot, D.make_aggs(specs), len(specs), part.n))
             self.keep.append(ctx)
         # ---- reused device buffers
         # ONE lookup buffer: every run rebuilds it in stream order, after the previous run's scan.  (Two
         # alternating buffers would keep both sets of evict_last lines next to the group tables, and a step
-        # would meet a lookup that the other buffer's protected lines have displaced.)
-        self.dn = dn
+        # would meet a lookup that the other buffer's protected lines have displaced.)  Directory, slots and
+        # the 4 flag words share it: one broadcast carries them all.
         self.slot_bits = _star_slot_bits(self.nslots - 1)
-        _, self.flags_off, words = _star_bitmap_words(self.prange, dn, self.slot_bits)
+        slots_off, self.flags_off, words = _star_bitmap_words(q.prange, q.dn, self.slot_bits)
         self.lookup = torch.empty(words, dtype=torch.int32, device=dev)
-        self.lk = _star_bitmap_lookup(self.lookup, self.pmin, self.prange, dn, self.slot_bits)
-        # group tables: ONE (re-initialised per run) on the NCCL / single-GPU path; enable_peer_merge()
+        self.lk = lk = L.StarLookup()
+        lk.dense, lk.dir, lk.kmin, lk.range, lk.slot_bits = 2, self.lookup.data_ptr(), q.pmin, q.prange, self.slot_bits
+        lk.lookup = self.lookup.data_ptr() + 4 * slots_off
+        # group tables: ONE (re-initialised per run) on the NCCL / single-GPU path; install_peer_merge()
         # replaces it with two in symmetric memory that alternate run by run
-        self.tabs = [GroupState(dev, self.nslots, self.plan, need_present=True,
-                                alloc=_padded_slots(self.nslots, sharded))]
-        self.refill = [self._refill_list(self.tabs[0].table)]
+        self.tabs = [GroupState(dev, self.nslots, q.plan, need_present=True,
+                                alloc=_padded_slots(self.nslots, q.sharded))]
         self.dirty = [False]      # a fresh table is already initialised
         self.peer = None          # per-table b2_peer_merge descriptors once enabled
         self.epoch = 0
         self.free = [None, None]  # event recorded at the end of run k, waited for before run k + 2 is issued
-        self.merge_bufs = {}      # presence / reduce-scatter outputs, reused run after run
+        self.merge_bufs = {} if cached else None   # presence / reduce-scatter outputs, reused run after run
         self.runs = 0
 
-    @staticmethod
-    def _refill_list(t: D.GroupTable):
-        """(tensor, initial value) of every array of the table: what a run has to restore first."""
-        out = []
-        for acc in t.acc:
-            if acc is not None:
-                out.append((acc, float(acc[0].item()) if acc.dtype == torch.float64 else int(acc[0].item())))
-        for cnt in t.cnt:
-            if cnt is not None:
-                out.append((cnt, 0))
-        if t.rows is not None:
-            out.append((t.rows, 0))
-        if t.present is not None:
-            out.append((t.present, 0))
-        return out
-
     def install_peer_merge(self, state):
-        self.tabs, self.refill, self.dirty, self.peer, self.arena, self.local_ready = state
+        self.tabs, self.dirty, self.peer, self.arena, self.local_ready = state
         stats["peer_merge_plans"] = stats.get("peer_merge_plans", 0) + 1
 
     def build_peer_merge(self):
@@ -1768,7 +1759,7 @@ class PreparedStar:
         arena = P.PeerArena(2 * per_table + 4 * P.PeerArena.ALIGN, dev)
         _, sig_off = arena.carve(L.MAX_PEERS, torch.int64, 0)
         chunk = alloc // size
-        tabs, refill, dirty, peer = [], [], [], []
+        tabs, dirty, peer = [], [], []
         local_ready = torch.zeros(1, dtype=torch.int64, device=dev)
         for _ in range(2):
             offs = {}
@@ -1778,7 +1769,7 @@ class PreparedStar:
                 offs[t.data_ptr()] = off
                 return t
 
-            gs = GroupState(dev, self.nslots, self.plan, need_present=True, alloc=alloc, new=new)
+            gs = GroupState(dev, self.nslots, self.q.plan, need_present=True, alloc=alloc, new=new)
             t = gs.table
             m = L.PeerMerge()
             m.world, m.rank, m.lo, m.count = size, rank, rank * chunk, chunk
@@ -1787,7 +1778,7 @@ class PreparedStar:
             for p_, b in enumerate(arena.base):
                 m.peer_base[p_] = b
             arrays, accs, cnts, rows = [], [], [], None      # arrays: (tensor, op) in the kernel's order
-            for ka, acc, cnt in zip(self.plan.kaggs, t.acc, t.cnt):
+            for ka, acc, cnt in zip(self.q.plan.kaggs, t.acc, t.cnt):
                 if acc is not None:
                     op = {L.AGG_MIN: L.PEER_MIN_I64, L.AGG_MAX: L.PEER_MAX_I64, L.AGG_AND: L.PEER_AND_I64,
                           L.AGG_OR: L.PEER_OR_I64, L.AGG_XOR: L.PEER_XOR_I64}.get(
@@ -1817,10 +1808,9 @@ class PreparedStar:
             view = SlotView(t.nslots, rank * chunk, chunk, [pick(a) for a in t.acc], [pick(c) for c in t.cnt],
                             pick(t.rows), "bytes", pres, dist="keyrange")
             tabs.append(gs)
-            refill.append(self._refill_list(t))
             dirty.append(False)
             peer.append((m, view))
-        return tabs, refill, dirty, peer, arena, local_ready
+        return tabs, dirty, peer, arena, local_ready
 
     @staticmethod
     def _resident_parts(table, needed):
@@ -1833,17 +1823,17 @@ class PreparedStar:
             for name in needed:
                 c = p[name]
                 if not isinstance(c, DeviceColumn):
-                    raise _NotPreparable()          # host-resident table: uploaded per query, classic path
+                    raise _NotPreparable()          # host-resident table: uploaded per query
                 cols[name] = c
             parts.append(Part(cols, n))
         return parts
 
-    @staticmethod
-    def _only_table_columns(ctx: "ScanCtx"):
-        if any(not k.startswith("col:") for k in ctx.index):
+    def _only_table_columns(self, ctx: "ScanCtx"):
+        if self.cached and any(not k.startswith("col:") for k in ctx.index):
             raise _NotPreparable()                  # computed inputs / mask predicates are evaluated per query
 
     def run(self, src) -> Part:
+        q = self.q
         i = self.runs & 1
         self.runs += 1
         buf = self.lookup
@@ -1860,11 +1850,12 @@ class PreparedStar:
         # nothing to gain: the scan kernels are persistent grids that fill every SM, so the build kernels
         # wait for a whole fact partition anyway, and the extra stream, communicator and events only add
         # cost.)
-        if self.owner:
+        if q.owner:
             with _Phase("build"):
-                _star_bitmap_build(buf, self.dim_launch, self.pmin, self.prange, self.gmin, self.nslots - 1,
-                                   self.dn, self.slot_bits, sp)
-        if self.bcast:
+                _star_bitmap_build(buf, self.dim_launch, q.pmin, q.prange, q.gmin, self.nslots - 1, q.dn,
+                                   self.slot_bits, sp)
+        if q.bcast:
+            # the build side crosses NVLink as the finished lookup (directory + slots), not as its columns
             with _Phase("bcast"):
                 P.broadcast_(buf, 0)
         # ---- probe side
@@ -1872,8 +1863,7 @@ class PreparedStar:
         t = self.tabs[ti].table
         with _Phase("scan"):
             if self.dirty[ti]:
-                for tensor, value in self.refill[ti]:
-                    tensor.fill_(value)
+                t.reset()
             self.dirty[ti] = True
             for scan, fk_slot, aggs_arr, naggs, n in self.fact_launch:
                 stats["launches"] += 1
@@ -1890,18 +1880,20 @@ class PreparedStar:
                 L.peer_merge(C.byref(m), sp)
                 _kernel_event_end(ev)
         else:
-            view = _merge_dense(t, self.plan, self.sharded, self.dev, keep=self.merge_bufs)
+            view = _merge_dense(t, q.plan, q.sharded, self.dev, keep=self.merge_bufs)
         stats["star_fused"] += 1
 
         def general():   # a duplicate build key showed up: the general path redoes the query
             stats["star_fused"] -= 1
             return run_aggregate(src, allow_fast=False)
 
-        out = _finalize_dense(view, self.gmin, self.gname, self.gexpr0, self.glog, self.plan, self.dev,
-                              key_nullable=self.gnull, check=buf[self.flags_off:], fallback=general)
-        done = torch.cuda.Event()
-        done.record(main)
-        self.free[i] = done
+        # the duplicate-key flags ride on the (deferred) host copy of the group count
+        out = _finalize_dense(view, q.gmin, src.group_cols[0], q.gexpr0, q.glog, q.plan, self.dev,
+                              key_nullable=q.gnull, check=buf[self.flags_off:], fallback=general)
+        if self.cached:          # a plan run once is never waited for
+            done = torch.cuda.Event()
+            done.record(main)
+            self.free[i] = done
         return out
 
 
@@ -1928,13 +1920,6 @@ def _star_bitmap_words(prange, dn, slot_bits):
     return slots, flags, flags + 4
 
 
-def _star_bitmap_lookup(buf, pmin, prange, dn, slot_bits):
-    lk = L.StarLookup()
-    lk.dense, lk.dir, lk.kmin, lk.range, lk.slot_bits = 2, buf.data_ptr(), pmin, prange, slot_bits
-    lk.lookup = buf.data_ptr() + 4 * _star_bitmap_words(prange, dn, slot_bits)[0]
-    return lk
-
-
 def _star_bitmap_build(buf, launches, pmin, prange, gmin, null_slot, dn, slot_bits, sp):
     """The ranked-bitmap lookup from (scan, pk slot, grp slot) of every dim partition, in stream order:
     zero the directory (with packed slots, the slot words too: FILL ORs into them) and flags, mark every
@@ -1958,8 +1943,9 @@ def _star_bitmap_build(buf, launches, pmin, prange, gmin, null_slot, dn, slot_bi
 def _star_dense_fast(src, fact, dim, fk_e, pk_e, gexprs, aggs, fact_pred, dim_pred, sharded, dev) -> Optional[Part]:
     """Star pipeline when the dimension side is a registered table whose join key and (single)
     group key are dense int64 columns: the ranked-bitmap lookup built from the dim partitions
-    (_star_bitmap_build), b2_star_agg per fact partition, one compaction at the end.  Returns None when the shape does not apply or a
-    duplicate build key shows up (the general path then takes over)."""
+    (_star_bitmap_build), b2_star_agg per fact partition, one compaction at the end -- a PreparedStar,
+    cached when its inputs allow it.  Returns None when the shape does not apply; a duplicate build key
+    hands the query to the general path."""
     if len(gexprs) != 1 or not isinstance(dim.source, TableSource) or not isinstance(pk_e, ColRef):
         return None
     ge = E.substitute(gexprs[0], dim.exprs)
@@ -1996,67 +1982,29 @@ def _star_dense_fast(src, fact, dim, fk_e, pk_e, gexprs, aggs, fact_pred, dim_pr
     fpred, fnever = simplify_pred(fact.pred + [E.substitute(p, fact.exprs) for p in fact_pred])
     if never or fnever:
         return None
-    nslots = grng + 1
-    if os.environ.get("B200SQL_NO_PREPARED") != "1":
-        prep = PreparedStar.get(src, fact, dim, fk_e, pk_e, ge, gexprs[0], aggs, fpred, dpred,
-                                (pmin, prange, gmin, grng, gnull, dn), owner, world > 1 and dist == "root", sharded, dev)
-        if prep is not None:
-            return prep.run(src)
-    # directory, slots and the 4 flag words share one buffer: one broadcast carries them all
-    slot_bits = _star_slot_bits(nslots - 1)
-    _, flags_off, words = _star_bitmap_words(prange, dn, slot_bits)
-    buf = torch.empty(words, dtype=torch.int32, device=dev)
-    flags = buf[flags_off:]
-    with _Phase("build"):
-        if owner:
-            needed: Set[str] = {pk_e.name, ge.name}
-            for p in dpred:
-                p.refs(needed)
-            launches, keep = [], []
-            for part in materialize(dim.source, needed):
-                if part.n == 0:
-                    continue
-                ctx = ScanCtx(part, dpred)
-                pk_slot, g_slot = ctx.slot(pk_e), ctx.slot(ge)     # slots first: scan() snapshots the columns
-                launches.append((ctx.scan(), pk_slot, g_slot))
-                keep.append(ctx)
-            _star_bitmap_build(buf, launches, pmin, prange, gmin, nslots - 1, dn, slot_bits, D.stream_ptr())
-    if world > 1 and dist == "root":
-        # the build side crosses NVLink as the finished lookup (directory + slots), not as its columns
-        with _Phase("bcast"):
-            P.broadcast_(buf, 0)
     plan = AggPlan([(E.substitute(e, fact.exprs) if e is not None else None, o, f) for e, o, f in aggs],
                    _nullable_fn(fact, sharded))
-    gs = GroupState(dev, nslots, plan, need_present=True, alloc=_padded_slots(nslots, sharded))
-    lk = _star_bitmap_lookup(buf, pmin, prange, dn, slot_bits)
-    needed = set(fk_e.refs())
+    dcols: Set[str] = {pk_e.name, ge.name}
+    for p in dpred:
+        p.refs(dcols)
+    fcols = set(fk_e.refs())
     for ka in plan.kaggs:
-        ka.expr.refs(needed)
+        ka.expr.refs(fcols)
     for p in fpred:
-        p.refs(needed)
-    with _Phase("scan"):
-        for part in materialize(fact.source, needed, pred=fpred):
-            if part.n == 0:
-                continue
-            ctx = ScanCtx(part, fpred)
-            fk_slot = ctx.slot(fk_e)
-            gs.bind(ctx)
-            stats["launches"] += 1
-            ev = _kernel_event_begin("b2_star_agg_kernel", part.n)
-            L.star_agg(C.byref(ctx.scan()), fk_slot, C.byref(lk), gs.table.aggs, len(gs.table.specs),
-                       C.byref(gs.table.state), D.stream_ptr())
-            _kernel_event_end(ev)
-    view = _merge_dense(gs.table, plan, sharded, dev)
+        p.refs(fcols)
     glog = dim.col_type(gexprs[0].name)[1] if isinstance(gexprs[0], ColRef) else "int64"
-    stats["star_fused"] += 1
-
-    def general():   # a duplicate build key showed up: the general path redoes the query
-        stats["star_fused"] -= 1
-        return run_aggregate(src, allow_fast=False)
-
-    # the duplicate-key flags ride on the (deferred) host copy of the group count
-    return _finalize_dense(view, gmin, src.group_cols[0], gexprs[0], glog, plan, dev, key_nullable=gnull,
-                           check=flags, fallback=general)
+    q = _DenseStar(fk_e, pk_e, ge, gexprs[0], glog, plan, dpred, fpred, dcols, fcols, pmin, prange, gmin, grng,
+                   gnull, dn, owner, world > 1 and dist == "root", sharded)
+    if os.environ.get("B200SQL_NO_PREPARED") != "1":
+        prep = PreparedStar.get(src, q, dim, fact, dev)
+        if prep is not None:
+            return prep.run(src)
+    # not preparable: a plan for this execution only, over uploaded host columns and evaluated inputs
+    with _Phase("build"):
+        dparts = materialize(dim.source, dcols) if owner else []
+    with _Phase("scan"):
+        fparts = materialize(fact.source, fcols, pred=fpred)
+    return PreparedStar(q, dparts, fparts, dev).run(src)
 
 
 def try_star(src: AggSource, child: LazyFrame, gexprs, aggs, pred, sharded, allow_fast=True) -> Optional[Part]:

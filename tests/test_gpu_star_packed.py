@@ -253,27 +253,38 @@ def test_c4_shape_prepared_twice(ng, bits):
 
 
 @pytest.mark.parametrize("ng,bits", C4_RANGES)
-def test_c4_shape_unprepared(ng, bits):
-    """the same query on the per-query path (fresh lookup buffer every time)"""
+def test_c4_shape_unprepared(ng, bits, monkeypatch):
+    """the same query on the per-query path (a plan built for one execution, fresh lookup buffer, then
+    dropped) issues the launches of the prepared plan and caches nothing; so does a computed aggregate
+    input over the same resident tables"""
     from dask_sql_b200 import Context, executor
     rng = np.random.default_rng(ng + 1)
     dim, fact = _c4(ng, rng)
-    old = os.environ.get("B200SQL_NO_PREPARED")
-    os.environ["B200SQL_NO_PREPARED"] = "1"
-    try:
-        c = Context()
-        c.create_table("fact", fact, npartitions=4, persist=True)
-        c.create_table("dim", dim, npartitions=2, persist=True)
-        before = executor.stats["star_fused"]
-        got = c.sql("SELECT d.grp, SUM(f.val) AS rev, COUNT(*) AS n FROM fact f JOIN dim d ON f.fk = d.pk "
-                    "WHERE f.x > 0 AND d.flag < 5 GROUP BY d.grp").compute()
-    finally:
-        if old is None:
-            os.environ.pop("B200SQL_NO_PREPARED", None)
-        else:
-            os.environ["B200SQL_NO_PREPARED"] = old
-    assert executor.stats["star_fused"] == before + 1
-    _check(got, _expected(fact, dim))
+    c = Context()
+    c.create_table("fact", fact, npartitions=4, persist=True)
+    c.create_table("dim", dim, npartitions=2, persist=True)
+    q = ("SELECT d.grp, SUM(f.val{}) AS rev, COUNT(*) AS n FROM fact f JOIN dim d ON f.fk = d.pk "
+         "WHERE f.x > 0 AND d.flag < 5 GROUP BY d.grp")
+    exp = _expected(fact, dim)
+
+    def run(sql):
+        live, fused, launches = list(executor.PreparedStar._live), executor.stats["star_fused"], \
+            executor.stats["launches"]
+        got = c.sql(sql).compute()
+        assert executor.stats["star_fused"] == fused + 1
+        return got, executor.PreparedStar._live == live, executor.stats["launches"] - launches
+
+    monkeypatch.setenv("B200SQL_NO_PREPARED", "1")
+    got, nothing_cached, unprepared = run(q.format(""))
+    _check(got, exp)
+    assert nothing_cached
+    monkeypatch.delenv("B200SQL_NO_PREPARED")
+    got, nothing_cached, prepared = run(q.format(""))
+    _check(got, exp)
+    assert not nothing_cached and prepared == unprepared
+    got, nothing_cached, _ = run(q.format(" * 2"))
+    _check(got.assign(rev=got["rev"] / 2), exp)
+    assert nothing_cached
 
 
 def test_packed_staged_pipeline():
