@@ -317,42 +317,126 @@ b2_star_build_scan_kernel(const __grid_constant__ b2_scan_t s, int pk_col, int g
       ld.template load<B2_GB_R>(grp_col, live, false, grp);
       uint32_t gnull = 0;
       if (gc.valid) gnull = live & ~b2_valid_bits<B2_GB_R>(gc.valid, ld.row0, live);
+      uint32_t pos[B2_GB_R];
+      int32_t v[B2_GB_R];
 #pragma unroll
       for (int j = 0; j < B2_GB_R; ++j) {
+        pos[j] = 0;
+        v[j] = 0;
         if (!((live >> j) & 1)) continue;
         const uint64_t d = (uint64_t)pk[j] - (uint64_t)pk_min;
         const uint64_t w = dir[d >> 5];
-        const uint32_t pos = (uint32_t)(w >> 32) + __popc((uint32_t)w & ((1u << (d & 31)) - 1));
-        const int32_t v = (gnull >> j) & 1 ? null_slot : (int32_t)(grp[j] - grp_min);
-        if (slot_bits == 32) {
-          static_cast<int32_t*>(slots)[pos] = v;
-        } else {
-          // The k entries of a word come from different dim rows, so the word is updated atomically, and
-          // the entry is REPLACED, not ORed in: two passing rows with the same pk share one directory bit
-          // and so one entry, and an OR of their slots could exceed null_slot and send the probe's atomics
-          // past the group table before the host reads the duplicate flag.  As with the 32-bit store, one
-          // of the two valid slots wins.  The first guess is the zeroed word.
-          const uint32_t q = b2_slot_word(pos, slot_bits);
-          const uint32_t sh = (pos - q * (64 / slot_bits)) * slot_bits;
-          unsigned long long* p = reinterpret_cast<unsigned long long*>(slots) + q;
-          const unsigned long long m = ((1ull << slot_bits) - 1) << sh;
-          const unsigned long long e = ((unsigned long long)(uint32_t)v << sh) & m;
-          unsigned long long old = 0, seen;
-          while ((seen = atomicCAS(p, old, (old & ~m) | e)) != old) old = seen;
+        pos[j] = (uint32_t)(w >> 32) + __popc((uint32_t)w & ((1u << (d & 31)) - 1));
+        v[j] = (gnull >> j) & 1 ? null_slot : (int32_t)(grp[j] - grp_min);
+      }
+      if (slot_bits == 32 || slot_bits == 16) {
+        // whole aligned int32 / halfword entries: a plain store, the last writer wins (16 bits: the little-
+        // endian halfword `pos` is bits [(pos mod 4) * 16, + 16) of word pos / 4)
+#pragma unroll
+        for (int j = 0; j < B2_GB_R; ++j) {
+          if (!((live >> j) & 1)) continue;
+          if (slot_bits == 32) static_cast<int32_t*>(slots)[pos[j]] = v[j];
+          else static_cast<uint16_t*>(slots)[pos[j]] = (uint16_t)v[j];
+        }
+      } else {
+        // 21 bits: the 3 entries of a word come from different dim rows, so the word is updated by CAS, and
+        // the entry is REPLACED, not ORed in: two passing rows with the same pk share one directory bit and
+        // so one entry, and an OR of their slots could exceed null_slot and send the probe's atomics past
+        // the group table before the host reads the duplicate flag.  As with the plain stores, one of the
+        // two valid slots wins.  The first guess is the zeroed word.  A round issues the CAS of every
+        // pending entry before looking at any result, and the next round retries only the entries that
+        // lost, each from the word its CAS returned: a lane waits for a few round trips to L2, not for
+        // one per entry and attempt.
+        unsigned long long e[B2_GB_R], old[B2_GB_R];
+        uint32_t q[B2_GB_R], sh[B2_GB_R];
+#pragma unroll
+        for (int j = 0; j < B2_GB_R; ++j) {
+          q[j] = b2_slot_word(pos[j], 21);
+          sh[j] = (pos[j] - q[j] * 3) * 21;
+          e[j] = ((unsigned long long)(uint32_t)v[j] & 0x1FFFFFull) << sh[j];
+          old[j] = 0;
+        }
+        unsigned long long* w = reinterpret_cast<unsigned long long*>(slots);
+        for (uint32_t pend = live; pend;) {
+          unsigned long long seen[B2_GB_R];
+#pragma unroll
+          for (int j = 0; j < B2_GB_R; ++j)
+            if ((pend >> j) & 1) seen[j] = atomicCAS(w + q[j], old[j], (old[j] & ~(0x1FFFFFull << sh[j])) | e[j]);
+#pragma unroll
+          for (int j = 0; j < B2_GB_R; ++j) {
+            if (!((pend >> j) & 1)) continue;
+            if (seen[j] == old[j]) pend &= ~(1u << j);
+            else old[j] = seen[j];
+          }
         }
       }
     }
   }
 }
 
-struct b2_scan_io_dir {
+// RANK over tiles of B2_RANK_TILE directory words, in three launches and without scratch memory:
+//   (a) b2_star_rank_tile_kernel: every tile's popcount total into the rank half of its first word;
+//   (b) b2_star_rank_carry_kernel: one block scans those totals in place into the tiles' offsets;
+//   (c) b2_star_rank_tile_kernel<true>: every tile scans its own popcounts from its offset and writes
+//       every rank.
+// MARK writes only the bit halves, and (a) stores the whole rank half of the words it uses, so nothing
+// has to be zeroed for the rank.  2048-word tiles put the C4 directory (10M keys, 312.5k words) on 153
+// blocks, all resident at once on an H100.
+#define B2_RANK_PER_THREAD 8
+#define B2_RANK_TILE (B2_BLOCK * B2_RANK_PER_THREAD)
+
+__device__ __forceinline__ uint32_t* b2_rank_half(uint64_t* dir, int64_t i) {
+  return reinterpret_cast<uint32_t*>(dir + i) + 1;   // little-endian: the high half of word i
+}
+
+template <bool WRITE>
+__global__ void __launch_bounds__(B2_BLOCK) b2_star_rank_tile_kernel(uint64_t* __restrict__ dir, int64_t nwords) {
+  __shared__ int warp_sums[B2_WARPS];
+  __shared__ uint32_t tile_off;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int64_t t0 = (int64_t)blockIdx.x * B2_RANK_TILE;
+  const int64_t i0 = t0 + (int64_t)threadIdx.x * B2_RANK_PER_THREAD;   // a thread's words are consecutive
+  if (WRITE && threadIdx.x == 0) tile_off = *b2_rank_half(dir, t0);
+  uint32_t bits[B2_RANK_PER_THREAD];
+  int tsum = 0;
+#pragma unroll
+  for (int k = 0; k < B2_RANK_PER_THREAD; ++k) {
+    bits[k] = i0 + k < nwords ? (uint32_t)dir[i0 + k] : 0u;
+    tsum += __popc(bits[k]);
+  }
+  int incl = tsum;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int t = __shfl_up_sync(FULL_MASK, incl, o);
+    if (lane >= o) incl += t;
+  }
+  if (lane == 31) warp_sums[warp] = incl;
+  __syncthreads();   // also orders thread 0's read of the tile offset before any write of the tile's ranks
+  if (!WRITE) {
+    if (threadIdx.x == 0) {
+      int total = 0;
+      for (int w = 0; w < B2_WARPS; ++w) total += warp_sums[w];
+      *b2_rank_half(dir, t0) = (uint32_t)total;
+    }
+    return;
+  }
+  uint32_t r = tile_off + (uint32_t)(incl - tsum);
+  for (int w = 0; w < warp; ++w) r += (uint32_t)warp_sums[w];
+#pragma unroll
+  for (int k = 0; k < B2_RANK_PER_THREAD; ++k) {
+    if (i0 + k < nwords) dir[i0 + k] = (uint64_t)bits[k] | ((uint64_t)r << 32);
+    r += __popc(bits[k]);
+  }
+}
+
+struct b2_scan_io_tile_off {
   uint64_t* dir;
-  __device__ int64_t get(int64_t i) const { return __popc((uint32_t)dir[i]); }
-  __device__ void put(int64_t i, int64_t v) const { dir[i] = (uint64_t)(uint32_t)dir[i] | ((uint64_t)v << 32); }
+  __device__ int64_t get(int64_t t) const { return *b2_rank_half(dir, t * B2_RANK_TILE); }
+  __device__ void put(int64_t t, int64_t v) const { *b2_rank_half(dir, t * B2_RANK_TILE) = (uint32_t)v; }
 };
 
-__global__ void __launch_bounds__(B2_SCAN_THREADS) b2_star_build_rank_kernel(uint64_t* __restrict__ dir, int64_t nwords) {
-  b2_block_exclusive_scan(b2_scan_io_dir{dir}, nwords);
+__global__ void __launch_bounds__(B2_SCAN_THREADS) b2_star_rank_carry_kernel(uint64_t* __restrict__ dir, int64_t ntiles) {
+  b2_block_exclusive_scan(b2_scan_io_tile_off{dir}, ntiles);
 }
 
 __global__ void __launch_bounds__(B2_BLOCK)
@@ -730,8 +814,14 @@ int32_t b2_star_build_mark(const b2_scan_t* scan, int32_t pk_col, int64_t pk_min
 int32_t b2_star_build_rank(uint64_t* dir, int64_t pk_range, void* stream) {
   B2_REQUIRE(dir, "null argument");
   B2_REQUIRE(pk_range > 0 && pk_range < ((int64_t)1 << 31), "bad range");
-  b2_star_build_rank_kernel<<<1, B2_SCAN_THREADS, 0, (cudaStream_t)stream>>>(dir, (pk_range + 31) / 32);
-  B2_CHECK_LAUNCH("b2_star_build_rank_kernel");
+  const int64_t nwords = (pk_range + 31) / 32;
+  const int64_t ntiles = (nwords + B2_RANK_TILE - 1) / B2_RANK_TILE;
+  b2_star_rank_tile_kernel<false><<<(unsigned)ntiles, B2_BLOCK, 0, (cudaStream_t)stream>>>(dir, nwords);
+  B2_CHECK_LAUNCH("b2_star_rank_tile_kernel<false>");
+  b2_star_rank_carry_kernel<<<1, B2_SCAN_THREADS, 0, (cudaStream_t)stream>>>(dir, ntiles);
+  B2_CHECK_LAUNCH("b2_star_rank_carry_kernel");
+  b2_star_rank_tile_kernel<true><<<(unsigned)ntiles, B2_BLOCK, 0, (cudaStream_t)stream>>>(dir, nwords);
+  B2_CHECK_LAUNCH("b2_star_rank_tile_kernel<true>");
   return B2_OK;
 }
 
