@@ -25,7 +25,9 @@ OP_ADD_I, OP_SUB_I, OP_MUL_I, OP_DIV_I, OP_NEG_I, OP_ABS_I, OP_MOD_I = 10, 11, 1
 OP_ADD_F, OP_SUB_F, OP_MUL_F, OP_DIV_F, OP_NEG_F, OP_ABS_F, OP_SQRT_F = 20, 21, 22, 23, 24, 25, 26
 OP_EQ_I, OP_EQ_F = 30, 40
 OP_AND, OP_OR, OP_NOT, OP_ISNULL_I, OP_ISNULL_F, OP_CASE, OP_FILLNA, OP_ORD2F = 50, 51, 52, 53, 54, 55, 56, 57
-OP_DATEPART, OP_ADDMONTHS = 60, 61
+OP_DATEPART, OP_ADDMONTHS, OP_MAP = 60, 61, 62
+STR_ILIKE = 1
+STR_LB_MATCH, STR_LB_ORDER = 0, 1
 # B2_OP_DATEPART fields (b200sql.h B2_DP_*)
 (DP_DAYS, DP_YEAR, DP_QUARTER, DP_MONTH, DP_DAY, DP_DOY, DP_DOW, DP_ISOWEEK, DP_HOUR, DP_MINUTE, DP_SECOND,
  DP_MILLISECOND, DP_MICROSECOND) = range(13)
@@ -202,6 +204,8 @@ _SIGS = {
     "b2_star_build_hash": [C.POINTER(Col), _P, C.c_int64, _P, _P, _P, C.c_int64, _P, _P],
     "b2_star_agg": [C.POINTER(Scan), C.c_int32, C.POINTER(StarLookup), C.POINTER(Agg), C.c_int32,
                     C.POINTER(AggState), _P],
+    "b2_str_like": [_P, _P, C.c_int64, _P, C.c_int64, C.c_uint32, C.c_int32, _P, _P],
+    "b2_str_lower_bound": [_P, _P, C.c_int64, _P, _P, C.c_int64, C.c_int32, _P, _P, _P],
 }
 
 EXPORTS = sorted(list(_SIGS) + ["b2_last_error", "b2_num_tiles", "b2_stats_ws_bytes", "b2_scan_agg_ws_bytes",
@@ -292,6 +296,8 @@ star_build_fill = _wrap("b2_star_build_fill")
 star_build_fill_packed = _wrap("b2_star_build_fill_packed")
 star_build_hash = _wrap("b2_star_build_hash")
 star_agg = _wrap("b2_star_agg")
+str_like = _wrap("b2_str_like")
+str_lower_bound = _wrap("b2_str_lower_bound")
 num_tiles = _lib.b2_num_tiles
 stats_ws_bytes = _lib.b2_stats_ws_bytes
 scan_agg_ws_bytes = _lib.b2_scan_agg_ws_bytes

@@ -72,11 +72,21 @@ class Context:
         persist=True uploads the columns to HBM once; persist=False (the reference's default:
         'the data will be lazily loaded') keeps them in pinned host memory and streams them to the
         GPU for every query.  kwargs: npartitions (default 1, pandaslike.py:26) and
-        distribution = 'local' | 'sharded' | 'replicated' | 'root' for multi-GPU jobs."""
+        distribution = 'local' | 'sharded' | 'replicated' | 'root' for multi-GPU jobs.
+
+        VARCHAR columns are stored as int64 codes into a sorted per-column dictionary.  They come from
+        input that is already dictionary-typed -- a pandas `category` column with string categories, an
+        Arrow `dictionary<int*, string>` column (chunks may carry different dictionaries), a Parquet
+        column read back as one -- or from `dictionary=["col", ...]`, which dictionary-encodes the named
+        plain string columns of any input (Parquet: read_dictionary, CSV: a dictionary column type).
+        Any other string column raises NotImplementedError.  VARCHAR results come back as `category`.
+        A VARCHAR column cannot be in a 'sharded' or 'root' table: each rank would build its own
+        dictionary."""
         logger.debug(f"Creating table: '{table_name}' of format type '{format}' in schema '{schema_name}'")
         schema_name = schema_name or self.schema_name
         npartitions = kwargs.pop("npartitions", 1)
         distribution = kwargs.pop("distribution", "local")
+        dictionary = list(kwargs.pop("dictionary", None) or ())
         filepath = None
         if isinstance(input_table, str) and not persist:
             import os
@@ -86,7 +96,8 @@ class Context:
                 # query and pruned by the pushed-down filters (table_scan.py:80-99, physical/utils/filter.py)
                 kwargs.pop("gpu", None)
                 filepath = input_table
-                input_table = ParquetTable(input_table, distribution, table_name, kwargs.pop("columns", None))
+                input_table = ParquetTable(input_table, distribution, table_name, kwargs.pop("columns", None),
+                                           dictionary)
                 if kwargs:
                     raise TypeError(f"unsupported options for reading {filepath!r}: {sorted(kwargs)}")
         if isinstance(input_table, LazyFrame):
@@ -99,17 +110,22 @@ class Context:
                     # storage location (input_utils/location.py:11-54): Parquet / CSV column chunks are
                     # read with pyarrow and laid out on the device without a pandas detour
                     from .table import read_location
-                    input_table = read_location(input_table, format, **kwargs)
+                    input_table = read_location(input_table, format, dictionary=dictionary, **kwargs)
                     kwargs = {}
                 if type(input_table).__module__.startswith("pyarrow") and hasattr(input_table, "column_names"):
                     from .table import arrow_columns
-                    columns = arrow_columns(input_table)            # pyarrow.Table: buffers used as they are
+                    columns = arrow_columns(input_table, dictionary)  # pyarrow.Table: buffers used as they are
                 elif isinstance(input_table, pd.DataFrame):
                     columns = {str(c): input_table[c] for c in input_table.columns}
                 elif isinstance(input_table, dict):
                     columns = {str(k): v for k, v in input_table.items()}
                 else:
                     raise NotImplementedError(f"cannot create a table from {type(input_table).__name__}")
+                for name in dictionary:
+                    if name not in columns:
+                        raise KeyError(f"dictionary=: no column {name!r}")
+                    if not hasattr(columns[name], "logical"):
+                        columns[name] = pd.Series(columns[name]).astype("category")
                 dev = self._torch_device() if persist else None
                 table = DeviceTable.from_columns(columns, npartitions, dev, persist, distribution, table_name)
             table.name = table_name

@@ -152,6 +152,13 @@ b2_expr_kernel(const __grid_constant__ b2_prog_t prog, const __grid_constant__ b
           --sp;
         } else if (op == B2_OP_DATEPART) {
           sv[sp - 1] = b2_datepart(sv[sp - 1], ins.a, ins.imm_i);
+        } else if (op == B2_OP_MAP) {
+          const b2_col_t& c = cols.c[ins.a];
+          const int64_t x = sv[sp - 1];
+          const bool hit = !sn[sp - 1] && x >= 0 && x < ins.imm_i && (!c.valid || b2_bit(c.valid, x));
+          sv[sp - 1] = !hit ? 0 : c.dtype == B2_U8 ? (int64_t) reinterpret_cast<const uint8_t*>(c.data)[x]
+                                                   : reinterpret_cast<const int64_t*>(c.data)[x];
+          sn[sp - 1] = !hit;
         } else if (op == B2_OP_ADDMONTHS) {
           // stack: x, n
           sv[sp - 2] = b2_addmonths(sv[sp - 2], sv[sp - 1], ins.imm_i, ins.a);
@@ -319,6 +326,13 @@ int32_t b2_expr_eval(const b2_prog_t* prog, const b2_col_t* cols, int32_t ncols,
         B2_REQUIRE(sp >= 2, "stack underflow");
         sp -= 1;
       }
+    }
+    else if (op == B2_OP_MAP) {
+      const int a = prog->code[i].a;
+      B2_REQUIRE(a >= 0 && a < ncols, "MAP of unknown column");
+      B2_REQUIRE(cols[a].dtype == B2_I64 || cols[a].dtype == B2_U8, "MAP table must be B2_I64 or B2_U8");
+      B2_REQUIRE(prog->code[i].imm_i >= 0, "MAP table length must be >= 0");
+      B2_REQUIRE(sp >= 1, "stack underflow");
     }
     else if (op == B2_OP_CASE) { B2_REQUIRE(sp >= 3, "stack underflow"); sp -= 2; }
     else { B2_REQUIRE(sp >= 2, "stack underflow"); sp -= 1; }

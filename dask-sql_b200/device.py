@@ -12,6 +12,7 @@ import numpy as np
 import torch
 
 from . import _lib as L
+from . import strings as S
 from . import temporal as T
 from .expr import int_literal_is_exact
 
@@ -188,6 +189,8 @@ def column_to_host(col: DeviceColumn):
         if not mask.any():
             mask = None
     lg = col.logical
+    if S.is_varchar(lg):
+        return S.to_host(vals, mask, lg)
     unit = T.unit_of(lg)
     if unit is not None:
         return T.to_host_array(vals, unit, mask)

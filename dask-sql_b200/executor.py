@@ -24,6 +24,7 @@ from . import _lib as L
 from . import device as D
 from . import expr as E
 from . import parallel as P
+from . import strings as S
 from .device import DeviceColumn, TermSpec, I64, F64, U8
 from .expr import Expr, ColRef, Lit, Call
 from .frame import LazyFrame, Source, TableSource, JoinSource, AggSource, SortSource, LimitSource
@@ -254,8 +255,9 @@ def eval_expr(part: Part, e: Expr) -> DeviceColumn:
     if isinstance(e, ColRef):
         return part[e.name]
     names = sorted(e.refs())
-    cols = [part[n] for n in names]
-    prog = E.compile_expr(e, names)
+    tables = E.map_tables(e)
+    cols = [part[n] for n in names] + [t.column(_dev()) for t in tables]
+    prog = E.compile_expr(e, names, tables)
     nullable = E.may_be_null(e, lambda n: part[n].valid is not None)
     stats["launches"] += 1
     out = D.expr_eval(prog, cols, part.n, nullable)
@@ -2036,8 +2038,8 @@ def try_star(src: AggSource, child: LazyFrame, gexprs, aggs, pred, sharded, allo
     if not isinstance(fact.source, TableSource):
         return None
     fk_e, pk_e = fact.exprs[fk_name], dim.exprs[pk_name]
-    if fk_e.dtype != I64 or pk_e.dtype != I64:
-        return None
+    if fk_e.dtype != I64 or pk_e.dtype != I64 or E.is_varchar(fk_e) or E.is_varchar(pk_e):
+        return None           # string keys take the general join, which reconciles the two dictionaries
     dev = _dev()
 
     # ---- fast path: dense join key and dense group key straight from a registered table: the
@@ -2215,7 +2217,7 @@ def try_join_agg(src: AggSource, child: LazyFrame, aggs, pred, sharded) -> Optio
     if not isinstance(probe.source, TableSource):
         return None
     pk_e, bk_e = probe.exprs[pkey], build.exprs[bkey]
-    if pk_e.dtype != I64 or bk_e.dtype != I64:
+    if pk_e.dtype != I64 or bk_e.dtype != I64 or E.is_varchar(pk_e) or E.is_varchar(bk_e):
         return None
     pnames, bnames = set(probe.columns), set(build.columns)
     probe_pred, build_pred = [], []
@@ -2345,6 +2347,10 @@ def run_join(js: JoinSource, needed: Set[str]) -> List[Part]:
     # key expressions; mixed int/float keys compare as float64 (pandas upcasts the same way)
     pk_exprs = [probe.exprs[k] for k in pkeys]
     bk_exprs = [build.exprs[k] for k in bkeys]
+    for i, (a, b) in enumerate(zip(pk_exprs, bk_exprs)):
+        if E.is_varchar(a) or E.is_varchar(b):
+            # VARCHAR keys of two dictionaries: the side with fewer rows is translated into the other's
+            pk_exprs[i], bk_exprs[i] = S.join_keys(a, b, estimated_rows(probe) <= estimated_rows(build))
     for i, (a, b) in enumerate(zip(pk_exprs, bk_exprs)):
         if a.dtype == U8:
             a = pk_exprs[i] = E.cast(a, I64)

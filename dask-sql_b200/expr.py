@@ -104,6 +104,7 @@ def as_expr(x) -> Expr:
 
 
 def cast(e: Expr, dtype: int) -> Expr:
+    _no_varchar("CAST", e)
     if e.dtype == dtype:
         if dtype == I64 and T.is_temporal(e.logical):     # a DATE / TIMESTAMP as BIGINT: its ticks
             return Lit(e.value, I64) if isinstance(e, Lit) else Call("cast", [e], I64)
@@ -128,7 +129,22 @@ def is_temporal(x) -> bool:
     return isinstance(x, (T.TScalar, T.Interval)) or (isinstance(x, Expr) and T.is_temporal(x.logical))
 
 
+def is_varchar(x) -> bool:
+    """A VARCHAR (dictionary-coded) expression."""
+    from . import strings as S
+    return isinstance(x, Expr) and S.is_varchar(x)
+
+
+def _no_varchar(what, *xs):
+    if any(is_varchar(x) for x in xs):
+        raise NotImplementedError(f"{what} of a VARCHAR: a string value can only be compared, matched with "
+                                  "[NOT] LIKE / ILIKE, grouped, sorted, joined on, counted and MIN / MAX-ed here")
+
+
 def binop(op: str, a, b) -> Expr:
+    if is_varchar(a) or is_varchar(b):
+        from . import strings as S
+        return S.binop(op, a, b)
     if is_temporal(a) or is_temporal(b):
         return T.binop(op, a, b)
     if op in _CMP:
@@ -156,6 +172,8 @@ def binop(op: str, a, b) -> Expr:
 
 def unop(op: str, a) -> Expr:
     a = as_expr(a)
+    if op != "isnull":
+        _no_varchar(op, a)
     if op == "neg":
         return Call("neg", [cast(a, I64) if a.dtype == U8 else a], F64 if a.dtype == F64 else I64)
     if op == "abs":
@@ -172,7 +190,11 @@ def unop(op: str, a) -> Expr:
 
 
 def case(cond, then, other) -> Expr:
+    if isinstance(then, str) or isinstance(other, str):
+        raise NotImplementedError("CASE with a string result: a VARCHAR value built from two sources is not "
+                                  "supported")
     cond, then, other = as_expr(cond), as_expr(then), as_expr(other)
+    _no_varchar("CASE", then, other)
     if is_temporal(then) or is_temporal(other):
         then, other = T.unify(then, other)
         return Call("case", [cast(cond, U8), then, other], I64, then.logical)
@@ -186,7 +208,11 @@ def case(cond, then, other) -> Expr:
 
 
 def fillna(a, fill) -> Expr:
+    if isinstance(fill, str):
+        raise NotImplementedError("COALESCE / fillna with a string: a VARCHAR value built from two sources is "
+                                  "not supported")
     a, fill = as_expr(a), as_expr(fill)
+    _no_varchar("COALESCE", a, fill)
     if is_temporal(a) or is_temporal(fill):
         a, fill = T.unify(a, fill)
         return Call("fillna", [a, fill], I64, a.logical)
@@ -257,9 +283,22 @@ def as_term(e: Expr) -> Optional[Tuple[str, int, object]]:
 # ---------------------------------------------------------------------------------------------
 # compilation to the postfix program of b2_expr_eval
 # ---------------------------------------------------------------------------------------------
+def map_tables(e: Expr, out=None) -> list:
+    """The per-entry tables (strings.MapTable) that `e`'s "map" nodes look up, in first-use order: the
+    program reads them as columns len(col_names), len(col_names) + 1, ..."""
+    out = [] if out is None else out
+    if isinstance(e, Call):
+        if e.op == "map" and not any(t is e.param for t in out):
+            out.append(e.param)
+        for a in e.args:
+            map_tables(a, out)
+    return out
+
+
 class _Compiler:
-    def __init__(self, col_index: Dict[str, int]):
+    def __init__(self, col_index: Dict[str, int], tables=()):
         self.col_index = col_index
+        self.tables = list(tables)
         self.code: List[Tuple[int, int, int, float]] = []
 
     def emit(self, op, a=0, imm_i=0, imm_f=0.0):
@@ -371,12 +410,20 @@ class _Compiler:
             self.visit(args[1])
             self.emit(L.OP_ADDMONTHS, a=to_last, imm_i=tps)
             return
+        if op == "map":
+            k = next((i for i, t in enumerate(self.tables) if t is e.param), None)
+            if k is None:
+                raise NotImplementedError("a map over a dictionary table needs the table among the program's columns")
+            self.visit(args[0])
+            self.emit(L.OP_MAP, a=len(self.col_index) + k, imm_i=len(e.param))
+            return
         raise NotImplementedError(f"expression operator {op}")
 
 
-def compile_expr(e: Expr, col_names: Sequence[str]) -> L.Prog:
-    """Compile `e` over the columns `col_names` (their order defines LOAD indices)."""
-    comp = _Compiler({n: i for i, n in enumerate(col_names)})
+def compile_expr(e: Expr, col_names: Sequence[str], tables=()) -> L.Prog:
+    """Compile `e` over the columns `col_names` (their order defines LOAD indices), followed by the
+    per-entry `tables` of its "map" nodes (map_tables(e))."""
+    comp = _Compiler({n: i for i, n in enumerate(col_names)}, tables)
     comp.visit(e)
     if len(comp.code) > L.MAX_PROG:
         raise NotImplementedError(f"expression needs {len(comp.code)} instructions (max {L.MAX_PROG})")
@@ -397,7 +444,7 @@ def may_be_null(e: Expr, col_nullable) -> bool:
         return e.value is None
     if e.op == "isnull":
         return False
-    if e.op in ("divt", "mod"):
+    if e.op in ("divt", "mod", "map"):
         return True
     if e.op == "cast" and e.dtype == I64 and e.args[0].dtype == F64:
         return True

@@ -83,6 +83,9 @@ class AggSource(Source):
                 self.schema[out] = (U8, "bool")
             else:
                 dt, lg = child.col_type(in_col)
+                if E.is_varchar(child.exprs[in_col]) and fn not in ("min", "max"):
+                    raise NotImplementedError(f"{fn.upper()} of a VARCHAR column: only COUNT, MIN and MAX aggregate "
+                                              "strings")
                 if T.is_temporal(lg) and fn not in ("min", "max"):
                     raise NotImplementedError(f"{fn.upper()} of a {T.sql_type_of(lg)} column: only COUNT, MIN and "
                                               "MAX aggregate dates and timestamps")
@@ -191,6 +194,10 @@ class LazySeries:
 
     def isin(self, values):
         vals = list(values)
+        if E.is_varchar(self.expr):      # absent literals match no row: only the codes of present ones remain
+            from . import strings as S
+            d = S.dictionary_of(self.expr)
+            vals = [v for v in vals if not isinstance(v, str) or d.code_of(v) is not None]
         if not vals:
             return self._wrap(Lit(False))
         out = None
@@ -199,6 +206,13 @@ class LazySeries:
             out = t if out is None else (out | t)
         # pandas isin never yields NULL
         return out.fillna(False)
+
+    def like(self, pattern: str, escape="\\", ilike=False):
+        """SQL [I]LIKE against a VARCHAR column (strings.like)"""
+        from . import strings as S
+        if not E.is_varchar(self.expr):
+            raise NotImplementedError(f"LIKE on a {self.expr.logical} operand: only VARCHAR columns match patterns")
+        return self._wrap(S.like(self.expr, pattern, escape, ilike))
 
     def where(self, cond, other=None):
         return self._wrap(E.case(self._other(cond), self.expr, self._other(other)))

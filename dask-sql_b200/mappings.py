@@ -65,6 +65,8 @@ def python_to_sql_type(python_type) -> SqlTypeName:
     """mappings.py:92-116.  datetime64[D] (and date32) is DATE, datetime64[s|ms|us|ns] is TIMESTAMP;
     time-zone-aware and timedelta types are not supported."""
     key = str(python_type)
+    if key == "category":             # dictionary-coded strings (strings.py)
+        return SqlTypeName.VARCHAR
     sql = T.sql_type_of(key)
     if sql is not None:
         return SqlTypeName(sql)

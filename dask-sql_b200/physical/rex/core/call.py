@@ -194,6 +194,26 @@ def _temporal(build, nstatic):
     return run
 
 
+def _like(ilike: bool):
+    """[NOT] LIKE / ILIKE with a literal pattern; the ESCAPE character defaults to a backslash, as in the
+    reference (call.py:414-416)."""
+    from .... import strings as S
+
+    def run(args, rex):
+        x, pattern = args
+        escape = getattr(rex, "value", None)
+        escape = "\\" if escape is None else escape
+        if x is None or pattern is None:
+            return None
+        if is_frame(x):
+            hit = x.like(pattern, escape, ilike)
+            return ~hit if rex.isNegated() else hit
+        if not isinstance(x, str):
+            raise NotImplementedError(f"LIKE on a {type(x).__name__} literal")
+        return S.like_host(x, pattern, escape, ilike) != bool(rex.isNegated())
+    return run
+
+
 _COMPARISONS = {"=": operator.eq, "!=": operator.ne, "<>": operator.ne, ">": operator.gt, ">=": operator.ge,
                 "<": operator.lt, "<=": operator.le}
 
@@ -221,6 +241,8 @@ OPERATORS.update({
     "cast": _cast,
     "between": _between,
     "in list": _in_list,
+    "like": _like(False),
+    "ilike": _like(True),
     # DATE / TIMESTAMP (the reference's names, call.py:1137-1155)
     "date_part": _temporal(T.extract, 1),
     "datepart": _temporal(T.extract, 1),

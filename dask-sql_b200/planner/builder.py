@@ -286,10 +286,20 @@ class Binder:
             return PyExpr("between", "BOOLEAN", args=[rec(e.e), rec(e.lo), rec(e.hi)], negated=e.negated)
         if k == "inlist":
             return PyExpr("inlist", "BOOLEAN", args=[rec(e.e)] + [rec(i) for i in e["items"]], negated=e.negated)
+        if k == "like":
+            x, pattern = rec(e.e), rec(e.pattern)
+            if pattern.kind != "literal" or not isinstance(pattern.value, (str, type(None))):
+                raise NotImplementedError("[NOT] LIKE / ILIKE takes a string literal pattern")
+            if x.sql_type not in ("VARCHAR", "NULL"):
+                self.err(f"{'ILIKE' if e.ilike else 'LIKE'} takes a VARCHAR operand, not {x.sql_type}")
+            return PyExpr("like", "BOOLEAN", name="ilike" if e.ilike else "like", args=[x, pattern],
+                          negated=e.negated, value=e.escape)
         if k == "cast":
             ty = _CAST_TYPES.get(e.type)
             if ty is None:
                 self.err(f"Unsupported CAST target type {e.type}")
+            if ty == "VARCHAR":
+                raise NotImplementedError("CAST to VARCHAR is not supported: VARCHAR columns are dictionary codes")
             return PyExpr("cast", ty, args=[rec(e.e)])
         if k == "case":
             args = []
@@ -318,6 +328,8 @@ class Binder:
                     self.err(f"{name} takes exactly one argument")
                 if any(a.contains_agg() for a in args):
                     self.err("Aggregate function calls cannot be nested")
+                if name not in ("COUNT", "MIN", "MAX") and any(a.sql_type == "VARCHAR" for a in args):
+                    raise NotImplementedError(f"{name} of a VARCHAR: only COUNT, MIN and MAX aggregate strings")
                 if name not in ("COUNT", "MIN", "MAX") and any(a.sql_type in _TEMPORAL for a in args):
                     raise NotImplementedError(f"{name} of a {args[0].sql_type}: only COUNT, MIN and MAX aggregate "
                                               "dates and timestamps")

@@ -99,7 +99,7 @@ AGG_FUNCS = {"SUM", "AVG", "COUNT", "MIN", "MAX", "MEAN", "STDDEV", "STDDEV_SAMP
 
 class PyExpr:
     """kind: column | literal | binary | not | isnull | isnotnull | negative | between | inlist |
-    cast | case | agg | alias | scalarfn | istrue"""
+    cast | case | agg | alias | scalarfn | istrue | like (name: like | ilike, value: the ESCAPE character)"""
 
     def __init__(self, kind, sql_type, **kw):
         self.kind = kind
@@ -179,6 +179,10 @@ class PyExpr:
         if k == "inlist":
             items = ", ".join(a.display() for a in self.args[1:])
             return f"{self.args[0].display()} {'NOT ' if self.negated else ''}IN ([{items}])"
+        if k == "like":
+            esc = f" ESCAPE '{self.value}'" if self.value is not None else ""
+            return (f"{self.args[0].display()} {'NOT ' if self.negated else ''}{self.name.upper()} "
+                    f"{self.args[1].display()}{esc}")
         if k == "cast":
             return f"CAST({self.args[0].display()} AS {_ARROW.get(self.sql_type, self.sql_type)})"
         if k == "case":
@@ -227,7 +231,7 @@ class PyExpr:
         return {"column": "Column", "literal": "Literal", "alias": "Alias", "agg": "AggregateFunction",
                 "binary": "BinaryExpr", "not": "Not", "isnull": "IsNull", "isnotnull": "IsNotNull",
                 "negative": "Negative", "between": "Between", "inlist": "InList", "cast": "Cast",
-                "case": "Case", "scalarfn": "ScalarFunction", "istrue": "IsTrue"}[self.kind]
+                "case": "Case", "scalarfn": "ScalarFunction", "istrue": "IsTrue", "like": "Like"}[self.kind]
 
     def column_name(self, rel=None) -> str:
         return self.display()

@@ -12,6 +12,7 @@ that crate cannot be built here (no rustc/cargo), so this is a small recursive-d
 
 Expressions: literals (incl. DATE '...', TIMESTAMP '...', INTERVAL '...' [unit]), [qualifier.]column,
 + - * / %, comparisons, AND OR NOT, IS [NOT] NULL, [NOT] BETWEEN, [NOT] IN (list), CAST(e AS type),
+e [NOT] LIKE | ILIKE 'pattern' [ESCAPE 'c'],
 CASE WHEN, EXTRACT(field FROM e), FLOOR / CEIL(e TO unit), function calls incl. aggregates with
 DISTINCT and FILTER (WHERE ...).
 
@@ -41,6 +42,9 @@ KEYWORDS = {"SELECT", "FROM", "WHERE", "GROUP", "BY", "HAVING", "ORDER", "LIMIT"
             "FIRST", "LAST", "WITH", "FILTER", "UNION", "ALL", "EXPLAIN", "SEMI", "ANTI", "USING"}
 
 
+_LIKE_WORDS = ("LIKE", "ILIKE", "SIMILAR")
+_STRING_FUNCS = {"CONCAT", "UPPER", "LOWER", "SUBSTRING", "SUBSTR", "TRIM", "LTRIM", "RTRIM", "BTRIM", "POSITION",
+                 "STRPOS", "CHAR_LENGTH", "CHARACTER_LENGTH", "LENGTH", "REPLACE", "INITCAP", "OVERLAY"}
 _TIME_UNITS = {"YEAR", "QUARTER", "MONTH", "WEEK", "DAY", "HOUR", "MINUTE", "SECOND", "MILLISECOND", "MICROSECOND",
                "NANOSECOND"}
 
@@ -404,6 +408,10 @@ class Parser:
                 e = self._between_or_in(e, True)
             elif self.at_kw("BETWEEN", "IN"):
                 e = self._between_or_in(e, False)
+            elif self.at_word(*_LIKE_WORDS) or (self.at_kw("NOT") and self.toks[self.i + 1].kind == "id"
+                                                and self.toks[self.i + 1].val.upper() in _LIKE_WORDS):
+                negated = bool(self.eat_kw("NOT"))
+                e = self._like(e, negated)
             else:
                 return e
 
@@ -423,8 +431,24 @@ class Parser:
         self.expect_op(")")
         return Node("inlist", e=e, items=items, negated=negated)
 
+    def _like(self, e, negated):
+        word = self.eat_word(*_LIKE_WORDS)
+        if word == "SIMILAR":
+            raise NotImplementedError("SIMILAR TO is not supported; use LIKE / ILIKE")
+        pattern = self.parse_add()
+        escape = None
+        if self.eat_word("ESCAPE"):
+            if self.cur.kind != "str" or len(self.cur.val) != 1:
+                self.error("ESCAPE takes a string of one character")
+            escape = self.cur.val
+            self.i += 1
+        return Node("like", e=e, pattern=pattern, escape=escape, negated=negated, ilike=word == "ILIKE")
+
     def parse_add(self):
         e = self.parse_mul()
+        if self.at_op("||"):
+            raise NotImplementedError("string concatenation (||) is not supported: VARCHAR values are dictionary "
+                                      "codes here")
         while self.at_op("+", "-"):
             op = self.eat_op("+", "-")
             e = Node("bin", op=op, l=e, r=self.parse_mul())
@@ -501,6 +525,9 @@ class Parser:
             unit = self.ident().upper() if self.cur.kind == "id" and self.cur.val.upper().rstrip("S") in _TIME_UNITS \
                 else None
             return Node("interval", value=nxt.val, unit=unit)
+        if t.kind == "id" and t.val.upper() in _STRING_FUNCS and nxt.kind == "op" and nxt.val == "(":
+            raise NotImplementedError(f"{t.val.upper()}: string functions are not supported; VARCHAR columns are "
+                                      "compared, matched with [NOT] LIKE / ILIKE, grouped, sorted and joined on")
         if t.kind == "id" and t.val.upper() == "EXTRACT" and nxt.kind == "op" and nxt.val == "(":
             self.i += 2                                   # EXTRACT(field FROM x)
             field = self.ident().upper()

@@ -12,6 +12,7 @@ from typing import Dict, List, Optional
 import numpy as np
 import torch
 
+from . import strings as S
 from . import temporal as T
 from .device import DeviceColumn, Stats, column_from_host, I64, F64, U8, _pack_valid
 
@@ -73,10 +74,22 @@ class ArrowColumn:
         return None if bits_set == n else out.view(np.int32)
 
 
-def _arrow_array_to_column(arr) -> ArrowColumn:
+def _varchar_column(codes, null, logical) -> ArrowColumn:
+    vb = None if null is None else np.packbits(~null, bitorder="little")
+    return ArrowColumn(codes, vb, logical)
+
+
+def _arrow_array_to_column(arr, name="", as_dictionary=False) -> ArrowColumn:
+    """as_dictionary: dictionary-encode a plain string column (create_table(dictionary=[...]))"""
     import pyarrow as pa
 
     t = arr.type
+    if S.is_string_dictionary_type(t) or (as_dictionary and S.is_string_type(t)):
+        return _varchar_column(*S.encode_arrow(arr))       # VARCHAR: codes into a sorted dictionary
+    if S.is_string_type(t):
+        raise S.plain_string_error(repr(name))
+    if isinstance(arr, pa.ChunkedArray):
+        arr = arr.chunk(0) if arr.num_chunks == 1 else pa.concat_arrays(arr.chunks)
     n = len(arr)
     # DATE: date32 (days) / date64 (ms -> days); TIMESTAMP: timestamp[unit] without a time zone
     date_or_ts = pa.types.is_date(t) or (pa.types.is_timestamp(t) and t.tz is None)
@@ -124,19 +137,23 @@ def _arrow_array_to_column(arr) -> ArrowColumn:
     raise NotImplementedError(f"column type {t} is outside the int64/float64/bool hot path of this layer")
 
 
-def arrow_columns(table) -> Dict[str, ArrowColumn]:
+def arrow_columns(table, dictionary=()) -> Dict[str, ArrowColumn]:
     """pyarrow.Table -> {name: ArrowColumn}.  Multi-chunk columns are concatenated once (Arrow
-    does that in C++); single-chunk columns are zero-copy views of the Arrow buffers."""
+    does that in C++); single-chunk columns are zero-copy views of the Arrow buffers.  String
+    dictionary columns, and the plain string columns named in `dictionary`, become VARCHAR codes."""
     import pyarrow as pa
 
     out = {}
     for name in table.column_names:
         col = table.column(name)
+        if S.is_string_dictionary_type(col.type) or (name in dictionary and S.is_string_type(col.type)):
+            out[str(name)] = _arrow_array_to_column(col, name, True)     # chunks may carry different dictionaries
+            continue
         arr = col.chunk(0) if col.num_chunks == 1 else (col.combine_chunks() if col.num_chunks else
                                                        pa.array([], type=col.type))
         if isinstance(arr, pa.ChunkedArray):
             arr = arr.chunk(0) if arr.num_chunks == 1 else pa.concat_arrays(arr.chunks)
-        out[str(name)] = _arrow_array_to_column(arr)
+        out[str(name)] = _arrow_array_to_column(arr, name)
     return out
 
 
@@ -157,15 +174,21 @@ def read_location(location: str, format: Optional[str] = None, **kwargs):
         format = ext or "parquet"
     format = format.lower()
     columns = kwargs.pop("columns", None)
+    dictionary = list(kwargs.pop("dictionary", None) or ())
     kwargs.pop("gpu", None)
     if kwargs:
         raise TypeError(f"unsupported options for reading {location!r}: {sorted(kwargs)}")
     if format == "parquet":
         import pyarrow.parquet as pq
-        return pq.read_table(location, columns=list(columns) if columns is not None else None)
+        return pq.read_table(location, columns=list(columns) if columns is not None else None,
+                             read_dictionary=dictionary or None)
     if format == "csv":
         import pyarrow.csv as pcsv
-        t = pcsv.read_csv(location)
+        conv = pcsv.ConvertOptions(auto_dict_encode=False)
+        if dictionary:
+            import pyarrow as pa
+            conv = pcsv.ConvertOptions(column_types={c: pa.dictionary(pa.int32(), pa.string()) for c in dictionary})
+        t = pcsv.read_csv(location, convert_options=conv)
         return t.select(list(columns)) if columns is not None else t
     raise AttributeError(f"Do not understand the input format {format!r} (supported here: parquet, csv)")
 
@@ -178,6 +201,8 @@ def _host_column(values, pin=True) -> HostColumn:
     words = None
     if isinstance(values, ArrowColumn):
         vals, logical, words = values.values, values.logical, values.valid_words()
+    elif isinstance(values, pd.Series) and isinstance(values.dtype, pd.CategoricalDtype):
+        vals, mask, logical = S.encode_pandas(values)
     elif isinstance(values, pd.Series):
         arr = values.array
         if isinstance(arr, pd.arrays.BooleanArray):
@@ -208,6 +233,8 @@ def _host_column(values, pin=True) -> HostColumn:
             vals, dt = vals.astype(np.int64, copy=False), I64
         elif kind == "f":
             vals, dt = vals.astype(np.float64, copy=False), F64
+        elif kind in "OSU" or logical in ("str", "string"):
+            raise S.plain_string_error(f"of dtype {logical}")
         else:
             raise NotImplementedError(
                 f"column dtype {logical} is outside the int64/float64/bool hot path of this layer")
@@ -291,6 +318,8 @@ class DeviceTable:
     def from_columns(cls, columns: Dict[str, object], npartitions=1, device=None, persist=True,
                      distribution="local", name=None):
         """columns: name -> pandas Series / numpy array / torch tensor (host or device)."""
+        import pandas as pd
+        columns = dict(columns)
         names = list(columns)
         n = len(next(iter(columns.values()))) if names else 0
         npartitions = max(1, min(int(npartitions), max(1, n)))
@@ -305,6 +334,8 @@ class DeviceTable:
             part = {}
             for nm in names:
                 v = columns[nm]
+                if isinstance(v, pd.Series) and isinstance(v.dtype, pd.CategoricalDtype):
+                    v = columns[nm] = _varchar_column(*S.encode_pandas(v))   # one dictionary for all partitions
                 if isinstance(v, torch.Tensor) and v.is_cuda:
                     dt = {torch.int64: I64, torch.float64: F64, torch.uint8: U8}[v.dtype]
                     part[nm] = DeviceColumn(v[lo:hi], None, dt)
@@ -313,7 +344,9 @@ class DeviceTable:
                 hc = _host_column(piece, pin=not persist)
                 part[nm] = hc.to_device(device) if persist else hc
             parts.append(part)
-        return cls(parts, distribution, name)
+        table = cls(parts, distribution, name)
+        S.check_distribution(distribution, table.schema())
+        return table
 
     @classmethod
     def from_pandas(cls, df, npartitions=1, device=None, persist=True, distribution="local", name=None):
@@ -354,7 +387,7 @@ class ParquetTable(DeviceTable):
     pruning is conservative and can only skip IO.  Decoded column chunks are kept (host memory) for the
     next query, like an OS page cache; `stats` tells how many row groups each scan skipped."""
 
-    def __init__(self, location: str, distribution="local", name=None, columns=None):
+    def __init__(self, location: str, distribution="local", name=None, columns=None, dictionary=()):
         import pyarrow.parquet as pq
         self.location = location
         self.file = pq.ParquetFile(location)
@@ -369,6 +402,14 @@ class ParquetTable(DeviceTable):
                 units[f.name] = "D"
             elif pa.types.is_timestamp(f.type) and f.type.tz is None:
                 units[f.name] = f.type.unit
+        # VARCHAR columns: read once here to fix the table's dictionary; every row group's chunk is
+        # remapped into it when the row group is read
+        self._dictionary = tuple(dictionary)
+        self._varchar = {}
+        for f in self.file.schema_arrow:
+            if f.name in self._names and (S.is_string_dictionary_type(f.type) or
+                                          (f.name in self._dictionary and S.is_string_type(f.type))):
+                self._varchar[f.name] = S.encode_arrow(self.file.read(columns=[f.name]).column(f.name))[2]
         self._groups = []                       # per row group: {"rows": n, "cols": {name: {"min","max","nulls","rows"} | None}}
         for g in range(md.num_row_groups):
             rg = md.row_group(g)
@@ -382,12 +423,15 @@ class ParquetTable(DeviceTable):
                     unit = units.get(nm)
                     if unit is not None:       # datetime.date / datetime statistics -> ticks of the column's unit
                         lo, hi = T.stat_to_ticks(lo, unit), T.stat_to_ticks(hi, unit)
+                    elif nm in self._varchar:  # string statistics -> code bounds (conservative if truncated)
+                        lo, hi = S.stat_to_codes(self._varchar[nm].dictionary, lo, hi)
                     cols[nm] = {"min": lo, "max": hi, "nulls": st.null_count, "rows": rg.num_rows}
                 else:
                     cols[nm] = None
             self._groups.append({"rows": rg.num_rows, "cols": cols})
         self._cache = {}                        # (row group, column) -> HostColumn
         self.stats = {"scans": 0, "row_groups_read": 0, "row_groups_skipped": 0}
+        S.check_distribution(distribution, [(n, None, lg) for n, lg in self._varchar.items()])
         self.distribution = distribution
         self.name = name
         self._schema = None
@@ -398,7 +442,9 @@ class ParquetTable(DeviceTable):
         """zero-row host columns: they carry every column's physical / logical type"""
         if self._proto is None:
             empty = self.file.schema_arrow.empty_table().select(self._names)
-            self._proto = {n: _host_column(c, pin=False) for n, c in arrow_columns(empty).items()}
+            self._proto = {n: _host_column(c, pin=False) for n, c in arrow_columns(empty, self._dictionary).items()}
+            for n, lg in self._varchar.items():
+                self._proto[n].logical = lg
         return self._proto
 
     def schema(self):
@@ -444,7 +490,10 @@ class ParquetTable(DeviceTable):
         key = (g, name)
         if key not in self._cache:
             t = self.file.read_row_group(g, columns=[name])
-            self._cache[key] = _host_column(arrow_columns(t)[name], pin=torch.cuda.is_available())
+            lg = self._varchar.get(name)
+            col = arrow_columns(t)[name] if lg is None else \
+                _varchar_column(*S.encode_into(t.column(name), lg))
+            self._cache[key] = _host_column(col, pin=torch.cuda.is_available())
         return self._cache[key]
 
     @property

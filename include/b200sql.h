@@ -196,6 +196,10 @@ typedef struct b2_prog {
 #define B2_DP_MILLISECOND 11   /* within the second, 0..999 */
 #define B2_DP_MICROSECOND 12   /* within the second, 0..999999 */
 #define B2_DP_NFIELDS     13
+/* pops code x, pushes cols[a][x]: a dictionary-entry table (B2_I64 or B2_U8) of imm_i entries, e.g. the
+ * b2_str_like result or a b2_str_lower_bound translation.  NULL x, x outside [0, imm_i), or an entry
+ * whose validity bit is clear gives NULL. */
+#define B2_OP_MAP       62
 
 /* ---- runtime --------------------------------------------------------------------- */
 const char* b2_last_error(void);
@@ -225,6 +229,23 @@ int32_t b2_col_stats(const b2_col_t* col, int64_t n, int64_t* d_out, void* ws, v
  * out_valid != NULL, the Arrow validity bitmap of the result ((n+31)/32 uint32 words). */
 int32_t b2_expr_eval(const b2_prog_t* prog, const b2_col_t* cols, int32_t ncols, int64_t n,
                      void* out_data, uint32_t* out_valid, void* stream);
+
+/* ---- VARCHAR dictionaries ---------------------------------------------------------- */
+/* A VARCHAR column is int64 codes into a dictionary sorted by UTF-8 bytes (so code order is string
+ * order): int64 offsets[ndict + 1] into uint8 chars.  These calls work once per dictionary entry. */
+#define B2_STR_ILIKE     1   /* b2_str_like flag: fold ASCII A-Z to a-z on both sides */
+/* out[e] = entry e matches the LIKE pattern (pattern[0..plen), UTF-8): '%' matches any sequence
+ * (newlines included), '_' exactly one code point; `escape` is a code point (0xFFFFFFFF = none)
+ * whose next code point is taken literally.  Every other byte is a literal. */
+int32_t b2_str_like(const int64_t* offsets, const uint8_t* chars, int64_t ndict, const uint8_t* pattern,
+                    int64_t plen, uint32_t escape, int32_t flags, uint8_t* out, void* stream);
+#define B2_STR_LB_MATCH  0   /* out[i] = code of B's entry i in A; validity bit cleared when A lacks it */
+#define B2_STR_LB_ORDER  1   /* out[i] = 2 * lower_bound - (absent ? 1 : 0): comparable with 2 * A's codes */
+/* For each entry of dictionary B, a binary search in sorted dictionary A.  out: int64[nb];
+ * out_valid: (nb + 31) / 32 words, required for B2_STR_LB_MATCH, may be NULL for B2_STR_LB_ORDER. */
+int32_t b2_str_lower_bound(const int64_t* a_offsets, const uint8_t* a_chars, int64_t na, const int64_t* b_offsets,
+                           const uint8_t* b_chars, int64_t nb, int32_t mode, int64_t* out, uint32_t* out_valid,
+                           void* stream);
 
 /* ---- filter ---------------------------------------------------------------------- */
 /* Global (no GROUP BY) aggregates over a filtered scan, no survivor materialisation.
