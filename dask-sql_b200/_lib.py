@@ -26,6 +26,10 @@ OP_ADD_F, OP_SUB_F, OP_MUL_F, OP_DIV_F, OP_NEG_F, OP_ABS_F, OP_SQRT_F = 20, 21, 
 OP_EQ_I, OP_EQ_F = 30, 40
 OP_AND, OP_OR, OP_NOT, OP_ISNULL_I, OP_ISNULL_F, OP_CASE, OP_FILLNA, OP_ORD2F = 50, 51, 52, 53, 54, 55, 56, 57
 OP_DATEPART, OP_ADDMONTHS, OP_MAP = 60, 61, 62
+OP_MATH_F, OP_MATH2_F, OP_POW_I = 63, 64, 65
+# B2_OP_MATH_F / B2_OP_MATH2_F functions (b200sql.h B2_FN_*)
+(FN_CEIL, FN_FLOOR, FN_TRUNC, FN_ROUND, FN_SIGN, FN_DEGREES, FN_RADIANS, FN_EXP, FN_LN, FN_LOG10, FN_CBRT, FN_SIN,
+ FN_COS, FN_TAN, FN_COT, FN_ASIN, FN_ACOS, FN_ATAN, FN_ATAN2, FN_POW, FN_MOD) = range(21)
 STR_ILIKE = 1
 STR_LB_MATCH, STR_LB_ORDER = 0, 1
 # B2_OP_DATEPART fields (b200sql.h B2_DP_*)

@@ -86,6 +86,60 @@ __device__ __noinline__ int64_t b2_addmonths(int64_t x, int64_t n, int64_t tps, 
   return (int64_t)((uint64_t)(first + d2 - 1) * (uint64_t)tpd + (uint64_t)tod);
 }
 
+// ---- numeric SQL functions (B2_OP_MATH_F / MATH2_F / POW_I) ---------------------------------
+// Out of line for the same reason as the calendar code.  The slow path of sin / cos / tan (argument
+// reduction of huge x) uses a 40 B local array; ptxas counts it in the kernel's frame, but only that path
+// touches it (DESIGN.md section 4).
+__device__ __noinline__ int64_t b2_math_f(int64_t bits, int fn, double f, int64_t div_first) {
+  const double x = __longlong_as_double(bits);
+  double r;
+  switch (fn) {
+    case B2_FN_CEIL:    r = ceil(x); break;
+    case B2_FN_FLOOR:   r = floor(x); break;
+    case B2_FN_TRUNC:   r = trunc(x); break;
+    case B2_FN_ROUND:   r = div_first ? rint(x / f) * f : rint(x * f) / f; break;
+    case B2_FN_SIGN:    r = x > 0.0 ? 1.0 : x < 0.0 ? -1.0 : x == 0.0 ? 0.0 : x; break;
+    case B2_FN_DEGREES: r = x * (180.0 / 3.141592653589793238462643383279502884); break;
+    case B2_FN_RADIANS: r = x * (3.141592653589793238462643383279502884 / 180.0); break;
+    case B2_FN_EXP:     r = exp(x); break;
+    case B2_FN_LN:      r = log(x); break;
+    case B2_FN_LOG10:   r = log10(x); break;
+    case B2_FN_CBRT:    r = cbrt(x); break;
+    case B2_FN_SIN:     r = sin(x); break;
+    case B2_FN_COS:     r = cos(x); break;
+    case B2_FN_TAN:     r = tan(x); break;
+    case B2_FN_COT:     r = 1.0 / tan(x); break;
+    case B2_FN_ASIN:    r = asin(x); break;
+    case B2_FN_ACOS:    r = acos(x); break;
+    default:            r = atan(x); break;   // B2_FN_ATAN (b2_expr_eval rejects other ids)
+  }
+  return __double_as_longlong(r);
+}
+
+__device__ __noinline__ int64_t b2_math2_f(int64_t xbits, int64_t ybits, int fn) {
+  const double x = __longlong_as_double(xbits), y = __longlong_as_double(ybits);
+  double r;
+  if (fn == B2_FN_ATAN2) r = atan2(x, y);
+  else if (fn == B2_FN_POW) r = pow(x, y);
+  else {                                       // B2_FN_MOD: NumPy's npy_divmod remainder
+    r = fmod(x, y);
+    if (y != 0.0) {
+      if (r != 0.0) { if ((y < 0.0) != (r < 0.0)) r += y; }
+      else r = copysign(0.0, y);
+    }
+  }
+  return __double_as_longlong(r);
+}
+
+__device__ __noinline__ int64_t b2_pow_i(int64_t x, int64_t y) {   // y >= 0; wraps like np.power
+  uint64_t base = (uint64_t)x, r = 1;
+  for (uint64_t e = (uint64_t)y; e; e >>= 1) {
+    if (e & 1) r *= base;
+    base *= base;
+  }
+  return (int64_t)r;
+}
+
 __global__ void __launch_bounds__(B2_BLOCK)
 b2_expr_kernel(const __grid_constant__ b2_prog_t prog, const __grid_constant__ b2_cols_arg cols,
                int64_t n, void* __restrict__ out_data, uint32_t* __restrict__ out_valid) {
@@ -159,6 +213,8 @@ b2_expr_kernel(const __grid_constant__ b2_prog_t prog, const __grid_constant__ b
           sv[sp - 1] = !hit ? 0 : c.dtype == B2_U8 ? (int64_t) reinterpret_cast<const uint8_t*>(c.data)[x]
                                                    : reinterpret_cast<const int64_t*>(c.data)[x];
           sn[sp - 1] = !hit;
+        } else if (op == B2_OP_MATH_F) {
+          sv[sp - 1] = b2_math_f(sv[sp - 1], ins.a, ins.imm_f, ins.imm_i);
         } else if (op == B2_OP_ADDMONTHS) {
           // stack: x, n
           sv[sp - 2] = b2_addmonths(sv[sp - 2], sv[sp - 1], ins.imm_i, ins.a);
@@ -200,6 +256,11 @@ b2_expr_kernel(const __grid_constant__ b2_prog_t prog, const __grid_constant__ b
           else if (op == B2_OP_SUB_F) r = __double_as_longlong(__longlong_as_double(a) - __longlong_as_double(b));
           else if (op == B2_OP_MUL_F) r = __double_as_longlong(__longlong_as_double(a) * __longlong_as_double(b));
           else if (op == B2_OP_DIV_F) r = __double_as_longlong(__longlong_as_double(a) / __longlong_as_double(b));
+          else if (op == B2_OP_MATH2_F) r = b2_math2_f(a, b, ins.a);
+          else if (op == B2_OP_POW_I) {  // np.power raises on a negative exponent: NULL here
+            if (b < 0) rn = true;
+            else r = b2_pow_i(a, b);
+          }
           sv[sp - 1] = r;
           sn[sp - 1] = rn;
         }
@@ -334,8 +395,20 @@ int32_t b2_expr_eval(const b2_prog_t* prog, const b2_col_t* cols, int32_t ncols,
       B2_REQUIRE(prog->code[i].imm_i >= 0, "MAP table length must be >= 0");
       B2_REQUIRE(sp >= 1, "stack underflow");
     }
+    else if (op == B2_OP_MATH_F) {
+      const int a = prog->code[i].a;
+      B2_REQUIRE(a >= 0 && a < B2_FN_ATAN2, "MATH_F: unknown function");
+      B2_REQUIRE(a != B2_FN_ROUND || prog->code[i].imm_i == 0 || prog->code[i].imm_i == 1,
+                 "MATH_F: ROUND's imm_i must be 0 or 1");
+      B2_REQUIRE(sp >= 1, "stack underflow");
+    }
     else if (op == B2_OP_CASE) { B2_REQUIRE(sp >= 3, "stack underflow"); sp -= 2; }
-    else { B2_REQUIRE(sp >= 2, "stack underflow"); sp -= 1; }
+    else {
+      if (op == B2_OP_MATH2_F)
+        B2_REQUIRE(prog->code[i].a >= B2_FN_ATAN2 && prog->code[i].a < B2_FN_NFUNCS, "MATH2_F: unknown function");
+      B2_REQUIRE(sp >= 2, "stack underflow");
+      sp -= 1;
+    }
     B2_REQUIRE(sp <= B2_STACK, "expression too deep");
   }
   B2_REQUIRE(sp == 1, "program must leave exactly one value");

@@ -189,6 +189,73 @@ def unop(op: str, a) -> Expr:
     raise NotImplementedError(f"operator {op}")
 
 
+# Numeric SQL functions under the reference's operator names (call.py:1091-1113), each with the NumPy call
+# the reference makes.  The device restates those calls (b200sql.h B2_OP_MATH_F / MATH2_F / POW_I); a call
+# on literals folds on the host through the NumPy call itself (math_fold).
+MATH_UNARY = {"ceil": (L.FN_CEIL, np.ceil), "floor": (L.FN_FLOOR, np.floor), "truncate": (L.FN_TRUNC, np.trunc),
+              "round": (L.FN_ROUND, np.round), "sign": (L.FN_SIGN, np.sign), "degrees": (L.FN_DEGREES, np.degrees),
+              "radians": (L.FN_RADIANS, np.radians), "exp": (L.FN_EXP, np.exp), "ln": (L.FN_LN, np.log),
+              "log10": (L.FN_LOG10, np.log10), "cbrt": (L.FN_CBRT, np.cbrt), "sin": (L.FN_SIN, np.sin),
+              "cos": (L.FN_COS, np.cos), "tan": (L.FN_TAN, np.tan), "cot": (L.FN_COT, lambda x: 1 / np.tan(x)),
+              "asin": (L.FN_ASIN, np.arcsin), "acos": (L.FN_ACOS, np.arccos), "atan": (L.FN_ATAN, np.arctan),
+              "sqrt": (None, np.sqrt)}
+MATH_BINARY = {"atan2": (L.FN_ATAN2, np.arctan2), "power": (L.FN_POW, np.power), "mod": (L.FN_MOD, np.mod)}
+
+
+def pow10(d: int) -> float:
+    """NumPy's power of ten for np.round(x, d) (numpy/_core/src/multiarray/calculation.c, power_of_ten):
+    a table up to 1e8, then repeated multiplication by 10 from 1e9 -- not always 10.0 ** d (d = 23, 25, ...)."""
+    if d < 9:
+        return float(10 ** d)
+    r = 1e9
+    for _ in range(d - 9):
+        r *= 10.0
+        if r == np.inf:
+            break
+    return r
+
+
+def math(name: str, args, digits: int = 0) -> Expr:
+    """The function `name` of MATH_UNARY / MATH_BINARY over expressions; `digits`: ROUND's second operand.
+    Every result is a DOUBLE except POWER of two integers (BIGINT, np.power's wrapping integer power)."""
+    args = [as_expr(a) for a in args]
+    _no_varchar(name.upper(), *args)
+    if name == "sqrt":
+        return unop("sqrt", args[0])
+    if name in MATH_UNARY:
+        fn = MATH_UNARY[name][0]
+        param = (fn, 0.0, 0)
+        if name == "round":       # np.round: rint(x * f) / f, or rint(x / f) * f for negative digits
+            param = (fn, pow10(abs(digits)), int(digits < 0))
+        return Call("math", [cast(args[0], F64)], F64, param=param)
+    x, y = args
+    ints = F64 not in (x.dtype, y.dtype)
+    if name == "mod":             # the integer modulo is floored like np.mod; either way a DOUBLE
+        return cast(binop("mod", x, y), F64) if ints else binop("mod", x, y)
+    if name == "power" and ints:
+        return Call("powi", [cast(x, I64), cast(y, I64)], I64)
+    return Call("math2", [cast(x, F64), cast(y, F64)], F64, param=MATH_BINARY[name][0])
+
+
+def math_fold(name: str, vals, digits: int = 0):
+    """`name` on host scalars (None is NULL), with the device's results: the NumPy call, except that an
+    integer POWER with a negative exponent (where NumPy raises) and an integer MOD by zero are NULL."""
+    if any(v is None for v in vals):
+        return None
+    ints = all(isinstance(v, (int, np.integer)) for v in vals)
+    with np.errstate(all="ignore"):
+        if name in MATH_BINARY and ints and name != "atan2":
+            x, y = (np.int64(v) for v in vals)
+            if name == "mod":
+                return None if y == 0 else float(np.mod(x, y))
+            return None if y < 0 else int(np.power(x, y))
+        xs = [np.float64(v) for v in vals]
+        if name == "round":
+            return float(np.round(xs[0], digits))
+        fn = MATH_UNARY[name][1] if name in MATH_UNARY else MATH_BINARY[name][1]
+        return float(fn(*xs))
+
+
 def case(cond, then, other) -> Expr:
     if isinstance(then, str) or isinstance(other, str):
         raise NotImplementedError("CASE with a string result: a VARCHAR value built from two sources is not "
@@ -340,11 +407,24 @@ class _Compiler:
             f = e.dtype == F64
             table = {"add": (L.OP_ADD_I, L.OP_ADD_F), "sub": (L.OP_SUB_I, L.OP_SUB_F),
                      "mul": (L.OP_MUL_I, L.OP_MUL_F), "truediv": (None, L.OP_DIV_F),
-                     "divt": (L.OP_DIV_I, None), "mod": (L.OP_MOD_I, None)}
+                     "divt": (L.OP_DIV_I, None), "mod": (L.OP_MOD_I, L.OP_MATH2_F)}
             code = table[op][1 if f else 0]
             if code is None:
                 raise NotImplementedError(f"{op} on {_DT_NAME[e.dtype]}")
-            self.emit(code)
+            self.emit(code, a=L.FN_MOD if code == L.OP_MATH2_F else 0)
+            return
+        if op == "math":
+            fn, f, div_first = e.param
+            self.visit(args[0])
+            self.emit(L.OP_MATH_F, a=fn, imm_i=div_first, imm_f=f)
+            return
+        if op in ("math2", "powi"):
+            self.visit(args[0])
+            self.visit(args[1])
+            if op == "math2":
+                self.emit(L.OP_MATH2_F, a=e.param)
+            else:
+                self.emit(L.OP_POW_I)
             return
         if op in _CMP:
             self.visit(args[0])
@@ -444,7 +524,7 @@ def may_be_null(e: Expr, col_nullable) -> bool:
         return e.value is None
     if e.op == "isnull":
         return False
-    if e.op in ("divt", "mod", "map"):
+    if e.op in ("divt", "mod", "map", "powi"):
         return True
     if e.op == "cast" and e.dtype == I64 and e.args[0].dtype == F64:
         return True

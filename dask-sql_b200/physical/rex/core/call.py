@@ -1,7 +1,7 @@
 """RexCall: SQL operator calls of the int64/float64/bool hot path (the reference's operator table is
 dask_sql/physical/rex/core/call.py:1047-1156; SURVEY 2 row 6 lists the rows in scope): comparisons,
 boolean logic, arithmetic, IS [NOT] NULL / TRUE / FALSE / UNKNOWN, BETWEEN, IN (list), CAST, CASE,
-unary minus, ABS.
+unary minus, ABS and the numeric functions (ROUND, CEIL / FLOOR, POWER, MOD, LN, SIN, ...).
 
 A value is either a LazySeries -- a device expression that has not run yet -- or a Python scalar
 (None is SQL NULL).  An operator here is a plain function  (operands, rex) -> value  that only
@@ -194,6 +194,27 @@ def _temporal(build, nstatic):
     return run
 
 
+def _math(name):
+    """Numeric function (expr.MATH_UNARY / MATH_BINARY); ROUND's optional second operand is its digits.
+    Literal operands fold on the host through the same NumPy call; a column builds the device expression."""
+    from .... import expr as E
+    from ....frame import LazySeries
+
+    def run(args, rex):
+        vals = list(args)
+        digits = vals.pop() if name == "round" and len(vals) == 2 else 0
+        if any(v is None for v in vals) or digits is None:
+            return None
+        frames = [v for v in vals if is_frame(v)]
+        if not frames:
+            return E.math_fold(name, vals, digits)
+        if any(f.source is not frames[0].source for f in frames):
+            raise ValueError("cannot combine columns of different frames without a join")
+        e = E.math(name, [v.expr if is_frame(v) else v for v in vals], digits)
+        return LazySeries(frames[0].source, frames[0].pred, e)
+    return run
+
+
 def _like(ilike: bool):
     """[NOT] LIKE / ILIKE with a literal pattern; the ESCAPE character defaults to a backslash, as in the
     reference (call.py:414-416)."""
@@ -254,6 +275,10 @@ OPERATORS.update({
     "timestampceil": _temporal(lambda x, unit: T.floor_ceil(x, unit, True), 0),
     "last_day": _temporal(lambda x: T.add_months_expr(x, 0, to_last=True), 0),
 })
+# numeric functions (call.py:1091-1113, and SQRT)
+OPERATORS.update({name: _math(name) for name in ("ceil", "floor", "truncate", "round", "sign", "degrees", "radians",
+                                                  "sqrt", "exp", "ln", "log10", "cbrt", "sin", "cos", "tan", "cot",
+                                                  "asin", "acos", "atan", "atan2", "power", "mod")})
 
 
 def _as_positional(fn):

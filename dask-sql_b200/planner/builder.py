@@ -352,8 +352,34 @@ class Binder:
             args = [rec(a) for a in e.args]
             if name == "ABS" and len(args) == 1:
                 return PyExpr("scalarfn", _norm_type(args[0].sql_type), name="abs", args=args)
+            if name in _MATH_UNARY + _MATH_BINARY:
+                return self._bind_math(name, args)
             self.err(f"Function {name} is outside the int64/float64 hot path of this layer")
         self.err(f"Unsupported expression {k}")
+
+    # -- numeric functions --------------------------------------------------------------------
+    def _bind_math(self, name, args) -> PyExpr:
+        """The numeric functions of the reference's operator table (call.py:1091-1113) and SQRT.  Result types:
+        DataFusion's built-ins, and the reference's UDFs, which return Float64 (src/sql.rs:316-325); POWER of
+        two integers stays BIGINT."""
+        arity = (1, 2) if name == "ROUND" else (2,) if name in _MATH_BINARY else (1,)
+        if len(args) not in arity:
+            self.err(f"{name} takes {' or '.join(map(str, arity))} argument(s), not {len(args)}")
+        values = args[:1] if name == "ROUND" else args
+        for a in values:
+            if _norm_type(a.sql_type) not in ("BIGINT", "DOUBLE", "NULL"):
+                self.err(f"{name} takes numeric arguments, not {a.sql_type}")
+        if name == "ROUND" and len(args) == 2:
+            d = args[1]
+            lit = d.args[0] if d.kind == "negative" else d
+            if lit.kind != "literal" or not isinstance(lit.value, int) or isinstance(lit.value, bool):
+                if d.kind != "literal" and _norm_type(d.sql_type) == "BIGINT":
+                    raise NotImplementedError("ROUND(x, d) takes its digits d as an integer literal only")
+                self.err(f"ROUND takes its digits as an integer literal, not {d.display()}")
+        ty = "DOUBLE"
+        if name == "POWER" and "DOUBLE" not in [_norm_type(a.sql_type) for a in args]:
+            ty = "BIGINT"
+        return PyExpr("scalarfn", ty, name=name.lower(), args=args)
 
     # -- DATE / TIMESTAMP ---------------------------------------------------------------------
     def _temporal_arith(self, op, l, r) -> str:
@@ -422,3 +448,6 @@ class Binder:
 
 _TEMPORAL_FUNCS = ("EXTRACT", "DATE_PART", "DATEPART", "YEAR", "TIMESTAMPADD", "TIMESTAMPDIFF", "TIMESTAMPFLOOR",
                    "TIMESTAMPCEIL", "LAST_DAY")
+_MATH_UNARY = ("CEIL", "FLOOR", "TRUNCATE", "ROUND", "SIGN", "DEGREES", "RADIANS", "SQRT", "EXP", "LN", "LOG10", "CBRT",
+               "SIN", "COS", "TAN", "COT", "ASIN", "ACOS", "ATAN")
+_MATH_BINARY = ("ATAN2", "POWER", "MOD")

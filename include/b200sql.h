@@ -200,6 +200,34 @@ typedef struct b2_prog {
  * b2_str_like result or a b2_str_lower_bound translation.  NULL x, x outside [0, imm_i), or an entry
  * whose validity bit is clear gives NULL. */
 #define B2_OP_MAP       62
+/* Numeric SQL functions on doubles, with NumPy's results (the reference calls NumPy,
+ * physical/rex/core/call.py:1091-1113); a NULL operand gives NULL, a domain error gives NaN / +-inf. */
+#define B2_OP_MATH_F    63  /* pops x, pushes function a (B2_FN_CEIL .. B2_FN_ATAN) of x.  B2_FN_ROUND: imm_f is the
+                               power of ten f; imm_i = 0: rint(x * f) / f, imm_i = 1: rint(x / f) * f */
+#define B2_OP_MATH2_F   64  /* pops y, x, pushes function a (B2_FN_ATAN2 .. B2_FN_MOD) of (x, y) */
+#define B2_OP_POW_I     65  /* pops y, x: x ** y on int64, wrapping modulo 2^64 (np.power); y < 0 -> NULL */
+#define B2_FN_CEIL     0   /* np.ceil */
+#define B2_FN_FLOOR    1   /* np.floor */
+#define B2_FN_TRUNC    2   /* np.trunc */
+#define B2_FN_ROUND    3   /* np.round(x, d), half to even; the host passes NumPy's power of ten for |d| */
+#define B2_FN_SIGN     4   /* np.sign: +-1.0, +0.0 for +-0, NaN for NaN */
+#define B2_FN_DEGREES  5   /* x * (180 / pi) */
+#define B2_FN_RADIANS  6   /* x * (pi / 180) */
+#define B2_FN_EXP      7
+#define B2_FN_LN       8
+#define B2_FN_LOG10    9
+#define B2_FN_CBRT    10
+#define B2_FN_SIN     11
+#define B2_FN_COS     12
+#define B2_FN_TAN     13
+#define B2_FN_COT     14   /* 1 / tan(x) */
+#define B2_FN_ASIN    15
+#define B2_FN_ACOS    16
+#define B2_FN_ATAN    17
+#define B2_FN_ATAN2   18   /* atan2(x, y): the first SQL argument is x */
+#define B2_FN_POW     19   /* C99 pow */
+#define B2_FN_MOD     20   /* np.mod: fmod(x, y) moved to y's sign, a zero result takes y's sign; x mod 0 = NaN */
+#define B2_FN_NFUNCS  21
 
 /* ---- runtime --------------------------------------------------------------------- */
 const char* b2_last_error(void);
