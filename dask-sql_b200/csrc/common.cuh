@@ -317,7 +317,7 @@ __device__ __forceinline__ uint32_t b2_cmp_batch_f(const int64_t (&raw)[R], doub
 }
 
 // ---------------------------------------------------------------------------------------
-// column loaders: where a batch's values come from
+// column loader and the tile loops that hand it to a batch body
 // ---------------------------------------------------------------------------------------
 struct b2_gld {  // straight from global memory
   const b2_scan_t* s;
@@ -327,30 +327,44 @@ struct b2_gld {  // straight from global memory
     b2_load_batch<R>(s->cols[col], row0, bits, full, raw);
   }
 };
-struct b2_sld {  // from the shared-memory tile staged by the TMA producer warp (pipeline.cuh)
-  const b2_scan_t* s;
-  int64_t row0;            // global row of this lane's first row (bitmaps, out_slot)
-  const uint8_t* stage;    // base of the current stage in shared memory
-  const int32_t* col_off;  // byte offset of each column's tile within a stage
-  int tile_off;            // this lane's first row within the tile
-  template <int R>
-  __device__ __forceinline__ void load(int col, uint32_t bits, bool full, int64_t (&raw)[R]) const {
-    if (s->cols[col].dtype == B2_U8) {
-      const uint8_t* p = stage + col_off[col] + tile_off;
-#pragma unroll
-      for (int j = 0; j < R; ++j) raw[j] = (int64_t)p[j * 32];
-    } else {
-      const int64_t* p = reinterpret_cast<const int64_t*>(stage + col_off[col]) + tile_off;
-#pragma unroll
-      for (int j = 0; j < R; ++j) raw[j] = p[j * 32];
-    }
+
+// body(ld) once per tile of B2_BLOCK x R rows, tiles grid-strided over the CTAs
+template <int R, class Body>
+__device__ __forceinline__ void b2_tile_direct(const b2_scan_t& s, Body&& body) {
+  const int tile_off = (threadIdx.x >> 5) * (32 * R) + (threadIdx.x & 31);
+  const int64_t tile = (int64_t)B2_BLOCK * R;
+  for (int64_t base = (int64_t)blockIdx.x * tile; base < s.n; base += (int64_t)gridDim.x * tile) {
+    const b2_gld ld{&s, base + tile_off};
+    body(ld);
   }
-};
+}
+
+// Tiles handed out IN ORDER by a global ticket instead of a fixed stride per CTA: the rows being
+// processed at any moment then form one contiguous window of (resident CTAs x tile) rows no matter how
+// unevenly the CTAs progress.  With a fixed stride a CTA that runs 10 % faster is 10 % of the input
+// ahead by the end -- fatal when the input is ordered so that a window should touch one L2-sized slice
+// of a table (partition.cuh).  *ticket must be 0 at launch.
+template <int R, class Body>
+__device__ __forceinline__ void b2_tile_ticket(const b2_scan_t& s, unsigned long long* __restrict__ ticket, Body&& body) {
+  __shared__ long long sh_tile;
+  const int tile_off = (threadIdx.x >> 5) * (32 * R) + (threadIdx.x & 31);
+  const int64_t tile = (int64_t)B2_BLOCK * R;
+  const int64_t ntiles = (s.n + tile - 1) / tile;
+  for (;;) {
+    if (threadIdx.x == 0) sh_tile = (long long)atomicAdd(ticket, 1ULL);
+    __syncthreads();
+    const int64_t t = sh_tile;
+    __syncthreads();
+    if (t >= ntiles) break;
+    const b2_gld ld{&s, t * tile + tile_off};
+    body(ld);
+  }
+}
 
 // Evaluate all predicate terms for the batch.  Returns the surviving row bits and whether the
 // batch is fully in bounds.
-template <int R, class LD>
-__device__ __forceinline__ uint32_t b2_eval_terms(const b2_scan_t& s, const LD& ld, bool& full, int& last_col,
+template <int R>
+__device__ __forceinline__ uint32_t b2_eval_terms(const b2_scan_t& s, const b2_gld& ld, bool& full, int& last_col,
                                                   int64_t (&raw)[R]) {
   // On return `raw` still holds the values of column `last_col` (the last term's column, -1 if
   // none) for the surviving rows: consumers that need the same column again (SUM(x) ... WHERE x > 0,
@@ -362,7 +376,7 @@ __device__ __forceinline__ uint32_t b2_eval_terms(const b2_scan_t& s, const LD& 
     const b2_term_t& tm = s.terms[t];
     const b2_col_t& c = s.cols[tm.col];
     const int op = tm.op;
-    ld.template load<R>(tm.col, bits, full, raw);
+    ld.load<R>(tm.col, bits, full, raw);
     last_col = tm.col;
     uint32_t ok;
     if (op == B2_IS_NULL || op == B2_IS_NOT_NULL) {
@@ -385,8 +399,8 @@ __device__ __forceinline__ uint32_t b2_eval_terms(const b2_scan_t& s, const LD& 
   }
   return bits;
 }
-template <int R, class LD>
-__device__ __forceinline__ uint32_t b2_eval_terms(const b2_scan_t& s, const LD& ld, bool& full) {
+template <int R>
+__device__ __forceinline__ uint32_t b2_eval_terms(const b2_scan_t& s, const b2_gld& ld, bool& full) {
   int last_col;
   int64_t raw[R];
   return b2_eval_terms<R>(s, ld, full, last_col, raw);
@@ -478,8 +492,8 @@ struct b2_aggs_arg {  // aggs passed by value in kernel params
 // load its input column for the contributing rows, drop NULLs, apply the atomics.
 // `pre` (optional): values of aggregate 0's input column already loaded by the caller for the rows
 // in `pre_bits` (a superset of the contributing rows), so that this load overlapped the slot lookup.
-template <int R, class LD>
-__device__ __forceinline__ void b2_apply_aggs(const b2_scan_t& s, const LD& ld, const b2_agg_t* __restrict__ aggs,
+template <int R>
+__device__ __forceinline__ void b2_apply_aggs(const b2_scan_t& s, const b2_gld& ld, const b2_agg_t* __restrict__ aggs,
                                               int naggs, const b2_aggstate_t& st,
                                               const int64_t (&slot)[R], const int64_t* pre = nullptr) {
   const int64_t row0 = ld.row0;
@@ -517,7 +531,7 @@ __device__ __forceinline__ void b2_apply_aggs(const b2_scan_t& s, const LD& ld, 
 #pragma unroll
       for (int j = 0; j < R; ++j) raw[j] = pre[j];
     } else {
-      ld.template load<R>(ag.col, live, false, raw);
+      ld.load<R>(ag.col, live, false, raw);
     }
     uint32_t ok = live;
     if (c.valid || c.dtype == B2_F64) ok &= ~b2_null_bits<R>(c, row0, live, raw);

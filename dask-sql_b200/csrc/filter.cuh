@@ -2,14 +2,13 @@
 // selection (count / scan / write+gather), gather.
 #pragma once
 #include "common.cuh"
-#include "pipeline.cuh"
 
 // =======================================================================================
 // fused filter + global aggregate   (SELECT SUM(x) FROM t WHERE x > 0)
 // each warp owns 32*R consecutive rows per step; lanes read 8-byte words 256 B apart per row
 // group so every warp-load is one fully coalesced 256-byte request.
 // =======================================================================================
-#define B2_AGG_R 16   // rows per lane per batch on the direct path (the staged path uses B2_PIPE_R)
+#define B2_AGG_R 16   // rows per lane per batch
 #define B2_AGG_ROWS_PER_BLOCK (B2_BLOCK * B2_AGG_R)
 
 struct b2_partial {
@@ -63,8 +62,8 @@ __device__ __forceinline__ int64_t b2_fold_batch(int64_t acc, const int64_t (&ra
 // run-time loop (no 8-way unrolled register file), the kind switch sits outside the row loop.
 // BITS: the instance that also folds AND / OR / XOR.  Those cases live in a kernel instance of their own:
 // inlined into the one every other query runs, they made C1 (a SUM) 4 % slower on H100.
-template <int R, bool BITS, class LD>
-__device__ __forceinline__ void b2_scan_agg_body(const b2_scan_t& s, const LD& ld, const b2_aggs_arg& aggs,
+template <int R, bool BITS>
+__device__ __forceinline__ void b2_scan_agg_body(const b2_scan_t& s, const b2_gld& ld, const b2_aggs_arg& aggs,
                                                  int64_t (*sh_acc)[B2_BLOCK], int32_t (*sh_cnt)[B2_BLOCK], int tid) {
   bool full;
   int cached_col;
@@ -82,7 +81,7 @@ __device__ __forceinline__ void b2_scan_agg_body(const b2_scan_t& s, const LD& l
 #pragma unroll
       for (int j = 0; j < R; ++j) raw[j] = cached[j];
     } else {
-      ld.template load<R>(ag.col, bits, full, raw);
+      ld.load<R>(ag.col, bits, full, raw);
     }
     uint32_t ok = bits;
     if (c.valid || c.dtype == B2_F64) ok &= ~b2_null_bits<R>(c, ld.row0, bits, raw);
@@ -110,10 +109,10 @@ __device__ __forceinline__ void b2_scan_agg_body(const b2_scan_t& s, const LD& l
   }
 }
 
-template <bool PIPE, bool BITS>
-__global__ void __launch_bounds__(PIPE ? B2_PIPE_THREADS : B2_BLOCK)
-b2_scan_agg_kernel(const __grid_constant__ b2_scan_t s, const __grid_constant__ b2_pipe_t pp,
-                   const __grid_constant__ b2_aggs_arg aggs, b2_partial* __restrict__ partials) {
+template <bool BITS>
+__global__ void __launch_bounds__(B2_BLOCK)
+b2_scan_agg_kernel(const __grid_constant__ b2_scan_t s, const __grid_constant__ b2_aggs_arg aggs,
+                   b2_partial* __restrict__ partials) {
   __shared__ int64_t sh_acc[B2_MAX_AGGS][B2_BLOCK];
   __shared__ int32_t sh_cnt[B2_MAX_AGGS][B2_BLOCK];
   const int tid = threadIdx.x;
@@ -123,8 +122,7 @@ b2_scan_agg_kernel(const __grid_constant__ b2_scan_t s, const __grid_constant__ 
       sh_cnt[a][tid] = 0;
     }
   }
-  if (PIPE) b2_tile_pipeline(s, pp, [&](const auto& ld) { b2_scan_agg_body<B2_PIPE_R, BITS>(s, ld, aggs, sh_acc, sh_cnt, tid); });
-  else b2_tile_direct<B2_AGG_R>(s, [&](const auto& ld) { b2_scan_agg_body<B2_AGG_R, BITS>(s, ld, aggs, sh_acc, sh_cnt, tid); });
+  b2_tile_direct<B2_AGG_R>(s, [&](const b2_gld& ld) { b2_scan_agg_body<B2_AGG_R, BITS>(s, ld, aggs, sh_acc, sh_cnt, tid); });
   __syncthreads();
   // block reduction in a fixed order: thread a folds the 256 per-thread slots of aggregate a.
   // (int32 per-thread counts cannot overflow: a thread sees < 2^31 rows of a < 2^31-row partition)
@@ -410,24 +408,14 @@ int32_t b2_scan_agg(const b2_scan_t* scan, const b2_agg_t* aggs, int32_t naggs, 
   if (rc) return rc;
   B2_REQUIRE(d_out_acc && d_out_cnt && ws, "null argument");
   cudaStream_t st = (cudaStream_t)stream;
-  b2_pipe_t pp;
-  b2_make_pipe(*scan, &pp);
   b2_partial* partials = reinterpret_cast<b2_partial*>(ws);
   bool bits = false;
   for (int a = 0; a < naggs; ++a) bits |= aa.a[a].op >= B2_AGG_AND;
-  int grid;
-  if (pp.enabled) {
-    auto k = bits ? b2_scan_agg_kernel<true, true> : b2_scan_agg_kernel<true, false>;
-    grid = b2_pipe_grid(k, pp, scan->n);
-    if (grid > B2_MAX_PARTIALS) grid = B2_MAX_PARTIALS;
-    k<<<grid, B2_PIPE_THREADS, pp.smem_bytes, st>>>(*scan, pp, aa, partials);
-  } else {
-    auto k = bits ? b2_scan_agg_kernel<false, true> : b2_scan_agg_kernel<false, false>;
-    int64_t nblk = (scan->n + B2_AGG_ROWS_PER_BLOCK - 1) / B2_AGG_ROWS_PER_BLOCK;
-    grid = b2_wave_grid(k, B2_BLOCK, nblk);
-    if (grid > B2_MAX_PARTIALS) grid = B2_MAX_PARTIALS;
-    k<<<grid, B2_BLOCK, 0, st>>>(*scan, pp, aa, partials);
-  }
+  auto k = bits ? b2_scan_agg_kernel<true> : b2_scan_agg_kernel<false>;
+  int64_t nblk = (scan->n + B2_AGG_ROWS_PER_BLOCK - 1) / B2_AGG_ROWS_PER_BLOCK;
+  int grid = b2_wave_grid(k, B2_BLOCK, nblk);
+  if (grid > B2_MAX_PARTIALS) grid = B2_MAX_PARTIALS;
+  k<<<grid, B2_BLOCK, 0, st>>>(*scan, aa, partials);
   B2_CHECK_LAUNCH("b2_scan_agg_kernel");
   if (naggs > 0) {
     b2_final_arg fa;

@@ -5,7 +5,6 @@
 // plus the fused star pipeline (filter -> key lookup -> aggregate).
 #pragma once
 #include "common.cuh"
-#include "pipeline.cuh"
 #include "warpagg.cuh"
 
 #define B2_GB_R 8
@@ -13,14 +12,14 @@
 #define B2_MAX_PROBE 1024
 
 // ---- dense ------------------------------------------------------------------------------
-template <int R, class LD>
-__device__ __forceinline__ void b2_dense_slots_of(const b2_scan_t& s, const LD& ld, int key_col, int64_t kmin,
+template <int R>
+__device__ __forceinline__ void b2_dense_slots_of(const b2_scan_t& s, const b2_gld& ld, int key_col, int64_t kmin,
                                                   int64_t nslots, int64_t (&slot)[R]) {
   const b2_col_t& kc = s.cols[key_col];
   bool full;
   const uint32_t bits = b2_eval_terms<R>(s, ld, full);
   int64_t key[R];
-  ld.template load<R>(key_col, bits, full, key);
+  ld.load<R>(key_col, bits, full, key);
   uint32_t kvalid = bits;
   if (kc.valid) kvalid = b2_valid_bits<R>(kc.valid, ld.row0, bits);
 #pragma unroll
@@ -36,22 +35,19 @@ __device__ __forceinline__ void b2_dense_slots_of(const b2_scan_t& s, const LD& 
   }
 }
 
-template <class LD>
-__device__ __forceinline__ void b2_dense_body(const b2_scan_t& s, const LD& ld, int key_col, int64_t kmin,
+__device__ __forceinline__ void b2_dense_body(const b2_scan_t& s, const b2_gld& ld, int key_col, int64_t kmin,
                                               int64_t nslots, const b2_aggs_arg& aggs, const b2_aggstate_t& st) {
   int64_t slot[B2_GB_R];
   b2_dense_slots_of<B2_GB_R>(s, ld, key_col, kmin, nslots, slot);
   b2_apply_aggs<B2_GB_R>(s, ld, aggs.a, aggs.n, st, slot);
 }
 
-template <bool PIPE>
-__global__ void __launch_bounds__(PIPE ? B2_PIPE_THREADS : B2_BLOCK)
-b2_groupby_dense_kernel(const __grid_constant__ b2_scan_t s, const __grid_constant__ b2_pipe_t pp, int key_col,
-                        int64_t kmin, int64_t nslots, const __grid_constant__ b2_aggs_arg aggs,
-                        const __grid_constant__ b2_aggstate_t st, unsigned long long* ticket) {
-  auto body = [&](const auto& ld) { b2_dense_body(s, ld, key_col, kmin, nslots, aggs, st); };
-  if (PIPE) b2_tile_pipeline(s, pp, body);
-  else if (ticket) b2_tile_ticket<B2_GB_R>(s, ticket, body);
+__global__ void __launch_bounds__(B2_BLOCK)
+b2_groupby_dense_kernel(const __grid_constant__ b2_scan_t s, int key_col, int64_t kmin, int64_t nslots,
+                        const __grid_constant__ b2_aggs_arg aggs, const __grid_constant__ b2_aggstate_t st,
+                        unsigned long long* ticket) {
+  auto body = [&](const b2_gld& ld) { b2_dense_body(s, ld, key_col, kmin, nslots, aggs, st); };
+  if (ticket) b2_tile_ticket<B2_GB_R>(s, ticket, body);
   else b2_tile_direct<B2_GB_R>(s, body);
 }
 
@@ -110,15 +106,14 @@ __device__ __forceinline__ int64_t b2_hash1_slot(int64_t* __restrict__ tk, int64
   return -1;
 }
 
-template <class LD>
-__device__ __forceinline__ void b2_hash1_body(const b2_scan_t& s, const LD& ld, int key_col, int64_t* __restrict__ tk,
+__device__ __forceinline__ void b2_hash1_body(const b2_scan_t& s, const b2_gld& ld, int key_col, int64_t* __restrict__ tk,
                                               int64_t cap, const b2_aggs_arg& aggs, const b2_aggstate_t& st,
                                               int32_t* __restrict__ flags) {
   const b2_col_t& kc = s.cols[key_col];
   bool full;
   const uint32_t bits = b2_eval_terms<B2_GB_R>(s, ld, full);
   int64_t key[B2_GB_R];
-  ld.template load<B2_GB_R>(key_col, bits, full, key);
+  ld.load<B2_GB_R>(key_col, bits, full, key);
   const uint32_t knull = b2_null_bits<B2_GB_R>(kc, ld.row0, bits, key);
   int64_t slot[B2_GB_R];
 #pragma unroll
@@ -134,14 +129,11 @@ __device__ __forceinline__ void b2_hash1_body(const b2_scan_t& s, const LD& ld, 
   b2_apply_aggs<B2_GB_R>(s, ld, aggs.a, aggs.n, st, slot);
 }
 
-template <bool PIPE>
-__global__ void __launch_bounds__(PIPE ? B2_PIPE_THREADS : B2_BLOCK)
-b2_groupby_hash1_kernel(const __grid_constant__ b2_scan_t s, const __grid_constant__ b2_pipe_t pp, int key_col,
-                        int64_t* __restrict__ tk, int64_t cap, const __grid_constant__ b2_aggs_arg aggs,
-                        const __grid_constant__ b2_aggstate_t st, int32_t* __restrict__ flags) {
-  auto body = [&](const auto& ld) { b2_hash1_body(s, ld, key_col, tk, cap, aggs, st, flags); };
-  if (PIPE) b2_tile_pipeline(s, pp, body);
-  else b2_tile_direct<B2_GB_R>(s, body);
+__global__ void __launch_bounds__(B2_BLOCK)
+b2_groupby_hash1_kernel(const __grid_constant__ b2_scan_t s, int key_col, int64_t* __restrict__ tk, int64_t cap,
+                        const __grid_constant__ b2_aggs_arg aggs, const __grid_constant__ b2_aggstate_t st,
+                        int32_t* __restrict__ flags) {
+  b2_tile_direct<B2_GB_R>(s, [&](const b2_gld& ld) { b2_hash1_body(s, ld, key_col, tk, cap, aggs, st, flags); });
 }
 
 // ---- hash, composite keys -------------------------------------------------------------------
@@ -190,8 +182,7 @@ __device__ __forceinline__ int64_t b2_hashk_slot(int64_t* __restrict__ tk, uint8
   return -1;
 }
 
-template <class LD>
-__device__ __forceinline__ void b2_hashk_body(const b2_scan_t& s, const LD& ld, const b2_keys_arg& keys,
+__device__ __forceinline__ void b2_hashk_body(const b2_scan_t& s, const b2_gld& ld, const b2_keys_arg& keys,
                                               int64_t* __restrict__ tk, uint8_t* __restrict__ tnull,
                                               int32_t* __restrict__ tstate, int64_t cap, const b2_aggs_arg& aggs,
                                               const b2_aggstate_t& st, int32_t* __restrict__ flags) {
@@ -203,7 +194,7 @@ __device__ __forceinline__ void b2_hashk_body(const b2_scan_t& s, const LD& ld, 
   for (int k = 0; k < B2_MAX_KEYS; ++k) {
     knull[k] = 0;
     if (k < keys.n) {
-      ld.template load<B2_GB_R>(keys.cols[k], bits, full, kv[k]);
+      ld.load<B2_GB_R>(keys.cols[k], bits, full, kv[k]);
       knull[k] = b2_null_bits<B2_GB_R>(s.cols[keys.cols[k]], ld.row0, bits, kv[k]);
     }
   }
@@ -229,16 +220,14 @@ __device__ __forceinline__ void b2_hashk_body(const b2_scan_t& s, const LD& ld, 
   b2_apply_aggs<B2_GB_R>(s, ld, aggs.a, aggs.n, st, slot);
 }
 
-template <bool PIPE>
-__global__ void __launch_bounds__(PIPE ? B2_PIPE_THREADS : B2_BLOCK)
-b2_groupby_hashk_kernel(const __grid_constant__ b2_scan_t s, const __grid_constant__ b2_pipe_t pp,
-                        const __grid_constant__ b2_keys_arg keys, int64_t* __restrict__ tk,
-                        uint8_t* __restrict__ tnull, int32_t* __restrict__ tstate, int64_t cap,
-                        const __grid_constant__ b2_aggs_arg aggs, const __grid_constant__ b2_aggstate_t st,
-                        int32_t* __restrict__ flags) {
-  auto body = [&](const auto& ld) { b2_hashk_body(s, ld, keys, tk, tnull, tstate, cap, aggs, st, flags); };
-  if (PIPE) b2_tile_pipeline(s, pp, body);
-  else b2_tile_direct<B2_GB_R>(s, body);
+__global__ void __launch_bounds__(B2_BLOCK)
+b2_groupby_hashk_kernel(const __grid_constant__ b2_scan_t s, const __grid_constant__ b2_keys_arg keys,
+                        int64_t* __restrict__ tk, uint8_t* __restrict__ tnull, int32_t* __restrict__ tstate,
+                        int64_t cap, const __grid_constant__ b2_aggs_arg aggs,
+                        const __grid_constant__ b2_aggstate_t st, int32_t* __restrict__ flags) {
+  b2_tile_direct<B2_GB_R>(s, [&](const b2_gld& ld) {
+    b2_hashk_body(s, ld, keys, tk, tnull, tstate, cap, aggs, st, flags);
+  });
 }
 
 // ---- fused star pipeline ----------------------------------------------------------------------
@@ -476,11 +465,11 @@ __device__ __forceinline__ int32_t b2_star_lookup(const b2_starlookup_t& lk, int
   return -1;
 }
 
-// rows per lane per batch of the direct star kernel: 16 rather than 8 or 4 although it halves occupancy,
-// for more independent loads in flight per thread.
+// rows per lane per batch of the star kernel: 16 rather than 8 or 4 although it halves occupancy, for
+// more independent loads in flight per thread.
 #define B2_STAR_R 16
-template <int R, class LD>
-__device__ __forceinline__ void b2_star_body(const b2_scan_t& s, const LD& ld, int fk_col, const b2_starlookup_t& lk,
+template <int R>
+__device__ __forceinline__ void b2_star_body(const b2_scan_t& s, const b2_gld& ld, int fk_col, const b2_starlookup_t& lk,
                                              const b2_aggs_arg& aggs, const b2_aggstate_t& st) {
   // Two memory round trips per batch instead of four:
   //   1. the join-key column is requested together with the predicate columns (its sectors are
@@ -492,7 +481,7 @@ __device__ __forceinline__ void b2_star_body(const b2_scan_t& s, const LD& ld, i
   bool full0;
   const uint32_t inb = b2_bounds_bits<R>(ld.row0, s.n, full0);
   int64_t key[R];
-  ld.template load<R>(fk_col, inb, full0, key);
+  ld.load<R>(fk_col, inb, full0, key);
   bool full;
   const uint32_t bits = b2_eval_terms<R>(s, ld, full);
   uint32_t live = bits;
@@ -512,7 +501,7 @@ __device__ __forceinline__ void b2_star_body(const b2_scan_t& s, const LD& ld, i
       const uint64_t d = (uint64_t)key[j] - (uint64_t)lk.kmin;
       w[j] = (((live >> j) & 1) && d < range) ? (uint64_t)b2_ld_keep_i64(reinterpret_cast<const int64_t*>(lk.dir) + (d >> 5)) : 0;
     }
-    if (prefetch) ld.template load<R>(aggs.a[0].col, live, false, pre);
+    if (prefetch) ld.load<R>(aggs.a[0].col, live, false, pre);
     const int sb = lk.slot_bits;   // 16, 21 or 32 (b2_star_agg normalises 0); uniform across the grid
     if (sb == 32) {
       // never a 64-bit read here: with an odd entry count it would run 4 bytes past the array
@@ -560,20 +549,17 @@ __device__ __forceinline__ void b2_star_body(const b2_scan_t& s, const LD& ld, i
       if (((live >> j) & 1) && key[j] != B2_EMPTY_KEY) found[j] = b2_star_lookup(lk, key[j]);
     }
   }
-  if (lk.dense != 2 && prefetch) ld.template load<R>(aggs.a[0].col, live, false, pre);
+  if (lk.dense != 2 && prefetch) ld.load<R>(aggs.a[0].col, live, false, pre);
 #pragma unroll
   for (int j = 0; j < R; ++j) slot[j] = found[j];
   // `pre` is passed as it is, never as a pointer chosen at run time: that would put it in local memory
   b2_apply_aggs<R>(s, ld, aggs.a, aggs.n, st, slot, pre);
 }
 
-template <bool PIPE>
-__global__ void __launch_bounds__(PIPE ? B2_PIPE_THREADS : B2_BLOCK)
-b2_star_agg_kernel(const __grid_constant__ b2_scan_t s, const __grid_constant__ b2_pipe_t pp, int fk_col,
-                   const __grid_constant__ b2_starlookup_t lk, const __grid_constant__ b2_aggs_arg aggs,
-                   const __grid_constant__ b2_aggstate_t st) {
-  if (PIPE) b2_tile_pipeline(s, pp, [&](const auto& ld) { b2_star_body<B2_PIPE_R>(s, ld, fk_col, lk, aggs, st); });
-  else b2_tile_direct<B2_STAR_R>(s, [&](const auto& ld) { b2_star_body<B2_STAR_R>(s, ld, fk_col, lk, aggs, st); });
+__global__ void __launch_bounds__(B2_BLOCK)
+b2_star_agg_kernel(const __grid_constant__ b2_scan_t s, int fk_col, const __grid_constant__ b2_starlookup_t lk,
+                   const __grid_constant__ b2_aggs_arg aggs, const __grid_constant__ b2_aggstate_t st) {
+  b2_tile_direct<B2_STAR_R>(s, [&](const b2_gld& ld) { b2_star_body<B2_STAR_R>(s, ld, fk_col, lk, aggs, st); });
 }
 
 extern "C" {
@@ -601,17 +587,9 @@ static int32_t b2_groupby_dense_impl(const b2_scan_t* scan, int32_t key_col, int
   B2_REQUIRE(scan->cols[key_col].dtype == B2_I64 || scan->cols[key_col].dtype == B2_U8, "dense keys must be integers");
   B2_REQUIRE(nslots >= 2, "nslots must cover the key range plus the NULL slot");
   if (scan->n == 0) return B2_OK;
-  b2_pipe_t pp;
-  b2_make_pipe(*scan, &pp);
-  if (ticket) pp.enabled = 0;
-  if (pp.enabled) {
-    int grid = b2_pipe_grid(b2_groupby_dense_kernel<true>, pp, scan->n);
-    b2_groupby_dense_kernel<true><<<grid, B2_PIPE_THREADS, pp.smem_bytes, (cudaStream_t)stream>>>(*scan, pp, key_col, kmin, nslots, aa, *st, nullptr);
-  } else {
-    int64_t nblk = (scan->n + B2_GB_ROWS_PER_BLOCK - 1) / B2_GB_ROWS_PER_BLOCK;
-    int grid = b2_wave_grid(b2_groupby_dense_kernel<false>, B2_BLOCK, nblk);
-    b2_groupby_dense_kernel<false><<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(*scan, pp, key_col, kmin, nslots, aa, *st, ticket);
-  }
+  int64_t nblk = (scan->n + B2_GB_ROWS_PER_BLOCK - 1) / B2_GB_ROWS_PER_BLOCK;
+  int grid = b2_wave_grid(b2_groupby_dense_kernel, B2_BLOCK, nblk);
+  b2_groupby_dense_kernel<<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(*scan, key_col, kmin, nslots, aa, *st, ticket);
   B2_CHECK_LAUNCH("b2_groupby_dense_kernel");
   return B2_OK;
 }
@@ -711,16 +689,9 @@ int32_t b2_groupby_hash1(const b2_scan_t* scan, int32_t key_col, int64_t* table_
   B2_REQUIRE(table_keys && d_flags, "null argument");
   B2_REQUIRE(b2_pow2(cap), "cap must be a power of two");
   if (scan->n == 0) return B2_OK;
-  b2_pipe_t pp;
-  b2_make_pipe(*scan, &pp);
-  if (pp.enabled) {
-    int grid = b2_pipe_grid(b2_groupby_hash1_kernel<true>, pp, scan->n);
-    b2_groupby_hash1_kernel<true><<<grid, B2_PIPE_THREADS, pp.smem_bytes, (cudaStream_t)stream>>>(*scan, pp, key_col, table_keys, cap, aa, *st, d_flags);
-  } else {
-    int64_t nblk = (scan->n + B2_GB_ROWS_PER_BLOCK - 1) / B2_GB_ROWS_PER_BLOCK;
-    int grid = b2_wave_grid(b2_groupby_hash1_kernel<false>, B2_BLOCK, nblk);
-    b2_groupby_hash1_kernel<false><<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(*scan, pp, key_col, table_keys, cap, aa, *st, d_flags);
-  }
+  int64_t nblk = (scan->n + B2_GB_ROWS_PER_BLOCK - 1) / B2_GB_ROWS_PER_BLOCK;
+  int grid = b2_wave_grid(b2_groupby_hash1_kernel, B2_BLOCK, nblk);
+  b2_groupby_hash1_kernel<<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(*scan, key_col, table_keys, cap, aa, *st, d_flags);
   B2_CHECK_LAUNCH("b2_groupby_hash1_kernel");
   return B2_OK;
 }
@@ -744,18 +715,10 @@ int32_t b2_groupby_hashk(const b2_scan_t* scan, const int32_t* key_cols, int32_t
     ka.cols[k] = key_cols[k];
   }
   if (scan->n == 0) return B2_OK;
-  b2_pipe_t pp;
-  b2_make_pipe(*scan, &pp);
-  if (pp.enabled) {
-    int grid = b2_pipe_grid(b2_groupby_hashk_kernel<true>, pp, scan->n);
-    b2_groupby_hashk_kernel<true><<<grid, B2_PIPE_THREADS, pp.smem_bytes, (cudaStream_t)stream>>>(*scan, pp, ka, table_keys, table_nulls,
-                                                                        table_state, cap, aa, *st, d_flags);
-  } else {
-    int64_t nblk = (scan->n + B2_GB_ROWS_PER_BLOCK - 1) / B2_GB_ROWS_PER_BLOCK;
-    int grid = b2_wave_grid(b2_groupby_hashk_kernel<false>, B2_BLOCK, nblk);
-    b2_groupby_hashk_kernel<false><<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(*scan, pp, ka, table_keys, table_nulls,
-                                                                        table_state, cap, aa, *st, d_flags);
-  }
+  int64_t nblk = (scan->n + B2_GB_ROWS_PER_BLOCK - 1) / B2_GB_ROWS_PER_BLOCK;
+  int grid = b2_wave_grid(b2_groupby_hashk_kernel, B2_BLOCK, nblk);
+  b2_groupby_hashk_kernel<<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(*scan, ka, table_keys, table_nulls, table_state, cap,
+                                                                       aa, *st, d_flags);
   B2_CHECK_LAUNCH("b2_groupby_hashk_kernel");
   return B2_OK;
 }
@@ -878,16 +841,9 @@ int32_t b2_star_agg(const b2_scan_t* scan, int32_t fk_col, const b2_starlookup_t
   else if (l.dense) B2_REQUIRE(l.lookup && l.range > 0, "bad dense lookup");
   else B2_REQUIRE(l.table_keys && l.table_slots && b2_pow2(l.cap), "bad hash lookup");
   if (scan->n == 0) return B2_OK;
-  b2_pipe_t pp;
-  b2_make_pipe(*scan, &pp);
-  if (pp.enabled) {
-    int grid = b2_pipe_grid(b2_star_agg_kernel<true>, pp, scan->n);
-    b2_star_agg_kernel<true><<<grid, B2_PIPE_THREADS, pp.smem_bytes, (cudaStream_t)stream>>>(*scan, pp, fk_col, l, aa, *st);
-  } else {
-    int64_t nblk = (scan->n + (int64_t)B2_BLOCK * B2_STAR_R - 1) / ((int64_t)B2_BLOCK * B2_STAR_R);
-    int grid = b2_wave_grid(b2_star_agg_kernel<false>, B2_BLOCK, nblk);
-    b2_star_agg_kernel<false><<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(*scan, pp, fk_col, l, aa, *st);
-  }
+  int64_t nblk = (scan->n + (int64_t)B2_BLOCK * B2_STAR_R - 1) / ((int64_t)B2_BLOCK * B2_STAR_R);
+  int grid = b2_wave_grid(b2_star_agg_kernel, B2_BLOCK, nblk);
+  b2_star_agg_kernel<<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(*scan, fk_col, l, aa, *st);
   B2_CHECK_LAUNCH("b2_star_agg_kernel");
   return B2_OK;
 }

@@ -206,121 +206,6 @@ b2_part_scatter_kernel(const __grid_constant__ b2_scan_t s, int key_col, int64_t
   }
 }
 
-// ---- warp-autonomous scatter ------------------------------------------------------------------------
-// The block-wide kernel above spends half its time in barriers (ncu r01: stall_barrier 52 %, five
-// __syncthreads per 2048-row tile, 152 thread-instructions per row).  Here ONE WARP owns a chunk of
-// 32*R consecutive rows end to end and only ever synchronises with itself (__syncwarp):
-//   1. slots of the chunk (predicate + key), carried values into registers -- all loads coalesced;
-//   2. rank inside the chunk = shared-memory atomicAdd on a warp-private histogram;
-//   3. exclusive scan of the histogram by shuffles; one global atomicAdd per non-empty (chunk, bucket)
-//      reserves the output range; base - prefix is kept so that  dst = basem[bucket] + p;
-//   4. rows are staged in bucket order in warp-private shared memory (key', values, bucket id);
-//   5. lanes walk the staged rows in order: consecutive lanes -> consecutive output rows of a bucket.
-// Shared memory per warp: 12 B x buckets + (10 + 8 NC) B x 32R rows; sized by the host (dynamic).
-template <int R, int NC>
-__global__ void __launch_bounds__(B2_BLOCK)
-b2_part_scatter_warp_kernel(const __grid_constant__ b2_scan_t s, int key_col, int64_t kmin, int64_t nslots, int shift,
-                            int nbuckets, int nb_pad, int64_t nchunks, unsigned long long* __restrict__ cursor,
-                            int64_t* __restrict__ out_key, const __grid_constant__ b2_partcarry_arg carry) {
-  constexpr int ROWS = 32 * R;
-  extern __shared__ __align__(16) uint8_t b2_part_smem[];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const size_t per_warp = (size_t)nb_pad * 12 + (size_t)ROWS * (8 + 2 + 2 + 8 * NC);
-  uint8_t* my = b2_part_smem + (size_t)warp * per_warp;
-  long long* basem = reinterpret_cast<long long*>(my);                       // [nb_pad] base - prefix
-  int64_t* st_key = reinterpret_cast<int64_t*>(my + (size_t)nb_pad * 8);     // [ROWS]
-  int64_t* st_val = st_key + ROWS;                                           // [NC][ROWS]
-  int* hist = reinterpret_cast<int*>(st_val + (size_t)NC * ROWS);            // [nb_pad] count, then prefix
-  uint16_t* st_bkt = reinterpret_cast<uint16_t*>(hist + nb_pad);             // [ROWS]
-  uint16_t* st_src = st_bkt + ROWS;                                          // [ROWS] row within the chunk
-  const int per = nb_pad >> 5;                                               // buckets per lane in the scan
-  const int64_t nwarps = (int64_t)gridDim.x * B2_WARPS;
-  unsigned long long* mycur = cursor + (size_t)(blockIdx.x % B2_PART_GROUPS) * nbuckets;   // this CTA's cursor group
-  for (int64_t chunk = (int64_t)blockIdx.x * B2_WARPS + warp; chunk < nchunks; chunk += nwarps) {
-    for (int b = lane; b < nb_pad; b += 32) hist[b] = 0;
-    __syncwarp();
-    const int64_t row0 = chunk * ROWS + lane;
-    int64_t slot[R];
-    b2_part_slots<R>(s, key_col, kmin, nslots, row0, slot);
-    uint32_t live = 0;
-#pragma unroll
-    for (int j = 0; j < R; ++j) live |= (uint32_t)(slot[j] >= 0) << j;
-    int64_t val[NC > 0 ? NC : 1][R];
-#pragma unroll
-    for (int c = 0; c < NC; ++c)
-      b2_load_batch64<R>(s.cols[carry.cols[c]].data, row0, live, false, val[c]);
-    int rank[R];
-#pragma unroll
-    for (int j = 0; j < R; ++j) rank[j] = (live >> j) & 1 ? atomicAdd(&hist[(int)(slot[j] >> shift)], 1) : 0;
-    __syncwarp();
-    // exclusive scan over the buckets: lane owns buckets [lane*per, lane*per + per)
-    int tsum = 0;
-    for (int k = 0; k < per; ++k) tsum += hist[lane * per + k];
-    int incl = tsum;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int t = __shfl_up_sync(FULL_MASK, incl, o);
-      if (lane >= o) incl += t;
-    }
-    const int total = __shfl_sync(FULL_MASK, incl, 31);
-    int run = incl - tsum;
-    for (int k = 0; k < per; ++k) {
-      const int b = lane * per + k;
-      const int c = hist[b];
-      hist[b] = run;
-      if (c) basem[b] = (long long)atomicAdd(mycur + b, (unsigned long long)c) - run;
-      run += c;
-    }
-    __syncwarp();
-#pragma unroll
-    for (int j = 0; j < R; ++j) {
-      if ((live >> j) & 1) {
-        const int b = (int)(slot[j] >> shift);
-        const int p = hist[b] + rank[j];
-        st_key[p] = kmin + slot[j];
-#pragma unroll
-        for (int c = 0; c < NC; ++c) st_val[c * ROWS + p] = val[c][j];
-        st_bkt[p] = (uint16_t)b;
-        st_src[p] = (uint16_t)(lane + j * 32);
-      }
-    }
-    __syncwarp();
-    const int64_t chunk_row0 = chunk * ROWS;
-    for (int p = lane; p < total; p += 32) {
-      const int64_t dst = basem[st_bkt[p]] + p;
-      b2_st_stream(out_key + dst, st_key[p]);
-#pragma unroll
-      for (int c = 0; c < NC; ++c) b2_st_stream(reinterpret_cast<int64_t*>(carry.out[c]) + dst, st_val[c * ROWS + p]);
-      for (int c = NC; c < carry.n; ++c) {   // columns beyond the staged ones: gathered from the chunk (L1/L2 hits)
-        const int64_t v = __ldg(reinterpret_cast<const long long*>(s.cols[carry.cols[c]].data) + chunk_row0 + st_src[p]);
-        b2_st_stream(reinterpret_cast<int64_t*>(carry.out[c]) + dst, v);
-      }
-    }
-    __syncwarp();   // the warp's shared arrays are reused by its next chunk
-  }
-}
-
-template <int R, int NC>
-static int32_t b2_launch_scatter_warp(const b2_scan_t* scan, int32_t key_col, int64_t kmin, int64_t nslots, int32_t shift,
-                                      int32_t nbuckets, unsigned long long* cursor, int64_t* out_key,
-                                      const b2_partcarry_arg& carry, cudaStream_t st) {
-  const int nb_pad = (nbuckets + 31) & ~31;
-  const size_t per_warp = (size_t)nb_pad * 12 + (size_t)(32 * R) * (8 + 2 + 2 + 8 * NC);
-  const size_t smem = per_warp * B2_WARPS;
-  auto kern = b2_part_scatter_warp_kernel<R, NC>;
-  if (smem > 48 * 1024) B2_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int occ = 1;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, B2_BLOCK, smem);
-  if (occ < 1) return b2_fail(B2_ERR_ARG, "range partition: %zu bytes of shared memory per CTA do not fit", smem);
-  static_assert(32 * R * B2_WARPS == B2_PART_TILE, "a CTA of the warp kernel covers exactly one histogram tile per step");
-  const int64_t nchunks = (scan->n + 32 * R - 1) / (32 * R);
-  const int grid = b2_part_grid((scan->n + B2_PART_TILE - 1) / B2_PART_TILE);
-  kern<<<grid, B2_BLOCK, smem, st>>>(*scan, key_col, kmin, nslots, shift, nbuckets, nb_pad, nchunks, cursor, out_key,
-                                          carry);
-  B2_CHECK_LAUNCH("b2_part_scatter_warp_kernel");
-  return B2_OK;
-}
-
 extern "C" {
 
 int64_t b2_range_partition_ws_bytes(int32_t nbuckets) {
@@ -378,24 +263,8 @@ int32_t b2_range_partition_scatter(const b2_scan_t* scan, int32_t key_col, int64
   const int64_t ntiles = (scan->n + B2_PART_TILE - 1) / B2_PART_TILE;
   if (ntiles <= 0) return B2_OK;
   int64_t* ws = reinterpret_cast<int64_t*>(d_ws);
-  // Two kernels, same results.  Default: the CTA-wide one -- a 2048-row tile puts ~20 rows into each of
-  // ~100 buckets, so its staged stores are runs of ~170 bytes; the warp-autonomous kernel has no block
-  // barrier but its 256-row chunks leave runs of ~20 bytes (partial sectors), and once the per-bucket
-  // cursors were split into B2_PART_GROUPS groups the barriers stopped being the limit, so the fuller
-  // sectors decide.  B200SQL_SCATTER=warp selects the latter (re-read per call so tests can switch
-  // in-process).
-  int variant = 0;
-  if (const char* e = getenv("B200SQL_SCATTER")) {
-    if (!strcmp(e, "warp")) variant = 8;
-  }
-  if (variant) {
-    unsigned long long* cur = reinterpret_cast<unsigned long long*>(ws + nbuckets + 1);
-    cudaStream_t st = (cudaStream_t)stream;
-    const int nc = ncarry >= 2 ? 2 : ncarry;
-    if (nc == 0) return b2_launch_scatter_warp<8, 0>(scan, key_col, kmin, nslots, shift, nbuckets, cur, out_key, carry, st);
-    if (nc == 1) return b2_launch_scatter_warp<8, 1>(scan, key_col, kmin, nslots, shift, nbuckets, cur, out_key, carry, st);
-    return b2_launch_scatter_warp<8, 2>(scan, key_col, kmin, nslots, shift, nbuckets, cur, out_key, carry, st);
-  }
+  // The scatter is CTA-wide so that its stores fill whole sectors: a 2048-row tile puts ~20 rows into each
+  // of ~100 buckets, so the staged stores of one bucket are a run of ~170 bytes.
   const int grid = b2_part_grid(ntiles);
   b2_part_scatter_kernel<<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(
       *scan, key_col, kmin, nslots, shift, nbuckets, ntiles, reinterpret_cast<unsigned long long*>(ws + nbuckets + 1),

@@ -138,8 +138,8 @@ __device__ __forceinline__ bool b2_batch_repeats(const int64_t (&slot)[R], int l
 }
 
 // The aggregated counterpart of b2_apply_aggs (same arguments, same results up to float summation order).
-template <int R, class LD>
-__device__ __forceinline__ void b2_apply_aggs_grouped(const b2_scan_t& s, const LD& ld, const b2_agg_t* __restrict__ aggs,
+template <int R>
+__device__ __forceinline__ void b2_apply_aggs_grouped(const b2_scan_t& s, const b2_gld& ld, const b2_agg_t* __restrict__ aggs,
                                                       int naggs, const b2_aggstate_t& st, const int64_t (&slot)[R],
                                                       const b2_hot_t& hot, const b2_hot_smem& hs) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -208,7 +208,7 @@ __device__ __forceinline__ void b2_apply_aggs_grouped(const b2_scan_t& s, const 
     if (ag.col < 0) continue;
     const b2_col_t& c = s.cols[ag.col];
     int64_t raw[R];
-    ld.template load<R>(ag.col, live, false, raw);
+    ld.load<R>(ag.col, live, false, raw);
     uint32_t ok = live;
     if (c.valid || c.dtype == B2_F64) ok &= ~b2_null_bits<R>(c, row0, live, raw);
     void* acc = st.acc[a];
@@ -470,8 +470,8 @@ __device__ __forceinline__ void b2_hh_batch(void* acc, int64_t* cnt, const int64
 }
 
 // b2_apply_aggs with the heavy hitters' rows diverted to the thread-private partials
-template <int R, class LD>
-__device__ __forceinline__ void b2_apply_aggs_hh(const b2_scan_t& s, const LD& ld, const b2_agg_t* __restrict__ aggs,
+template <int R>
+__device__ __forceinline__ void b2_apply_aggs_hh(const b2_scan_t& s, const b2_gld& ld, const b2_agg_t* __restrict__ aggs,
                                                  int naggs, const b2_aggstate_t& st, const int64_t (&slot)[R],
                                                  const b2_hot_t& hot, const b2_hh_smem& hs) {
   const int64_t row0 = ld.row0;
@@ -511,7 +511,7 @@ __device__ __forceinline__ void b2_apply_aggs_hh(const b2_scan_t& s, const LD& l
     if (ag.col < 0) continue;
     const b2_col_t& c = s.cols[ag.col];
     int64_t raw[R];
-    ld.template load<R>(ag.col, live, false, raw);
+    ld.load<R>(ag.col, live, false, raw);
     uint32_t ok = live;
     if (c.valid || c.dtype == B2_F64) ok &= ~b2_null_bits<R>(c, row0, live, raw);
     void* acc = st.acc[a];

@@ -218,7 +218,7 @@ static void star_mix(int sms) {
   fill_rows<<<sms * 8, 256>>>(fk, x, val, nrows, nkeys);
   fill_dir<<<sms * 8, 256>>>(dir, nwords);
   CK(cudaDeviceSynchronize());
-  const int grid = sms * 2;   // 2 CTAs of 256 threads per SM, as b2_star_agg_kernel<false> at 128 registers
+  const int grid = sms * 2;   // 2 CTAs of 256 threads per SM, as b2_star_agg_kernel at 128 registers
   for (int rep = 0; rep < 3; ++rep) {   // the three widths alternate, so that drift hits all of them alike
     for (int sb : {32, 21, 16}) {
       float ms;

@@ -11,17 +11,15 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "dask-sql_b200", "libb200sql.so")
 OUT = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "build", "sass")
 WANT = {
-    "star_agg": r"b2_star_agg_kernelILb0E",
+    "star_agg": r"b2_star_agg_kernel",
     "join_stream": r"b2_join_stream_kernelILb1ELi3ELb1ELb1E",
     "join_agg_fast": r"b2_join_agg_fast_kernelILb1ELi0E",
-    "part_scatter_warp": r"b2_part_scatter_warp_kernelILi8ELi1E",
     "part_scatter_block": r"b2_part_scatter_kernel",
     "peer_merge_w8": r"b2_peer_merge_kernelILi8E",
-    "groupby_dense": r"b2_groupby_dense_kernelILb0E",
+    "groupby_dense": r"b2_groupby_dense_kernel",
     "groupby_dense_hh": r"b2_groupby_dense_hh_kernel",
     "groupby_dense_grouped": r"b2_groupby_dense_grouped_kernel",
-    "scan_agg": r"b2_scan_agg_kernelILb0ELb0E",
-    "scan_agg_tma": r"b2_scan_agg_kernelILb1ELb0E",
+    "scan_agg": r"b2_scan_agg_kernelILb0E",
 }
 INTERESTING = re.compile(r"\b(LDG|STG|REDG|ATOMG|ATOMS|ATOM|RED|LDS|STS|MATCH|VOTE|SHFL|REDUX|UBLKCP|SYNCS|BAR|CCTL|LDGSTS|UTMALDG|LD|ST|NANOSLEEP|MEMBAR|ERRBAR)\b")
 

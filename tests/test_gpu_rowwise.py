@@ -377,8 +377,7 @@ def _term_column(dtype, nullable, n, rng):
 @pytest.mark.parametrize("dtype", [R.I64, R.F64, R.U8], ids=["i64", "f64", "u8"])
 def test_terms_every_op_and_literal(dtype, nullable):
     """one term at a time: every operator x every literal of the pool x as_f64, checked through the
-    selection and, with the term's column aggregated, through b2_scan_agg (n >= 4 x 2048: the staged
-    instance takes its TMA path, plus a 37-row tail)"""
+    selection and, with the term's column aggregated, through b2_scan_agg (whole tiles plus a 37-row tail)"""
     rng = np.random.default_rng(10 * dtype + nullable)
     n = 8229
     other = _column(rng.integers(-100, 100, n), R.I64, (rng.random(n) < 0.3) if nullable else None)
@@ -440,8 +439,7 @@ def test_terms_conjunctions_select(n, nterms):
 @pytest.mark.parametrize("n", [0] + SIZES)
 def test_terms_conjunctions_scan_agg(n, nterms):
     """COUNT(*) and exact aggregates over the LAST term's column (whose values b2_scan_agg_body reuses from
-    the predicate's registers) and over an EARLIER term's column (re-loaded).  At n >= 8192 the staged
-    instance (B200SQL_PIPELINE=1, tests/test_gpu_pipeline.py) takes its TMA path."""
+    the predicate's registers) and over an EARLIER term's column (re-loaded)."""
     rng = np.random.default_rng(2000 * nterms + n)
     cols = _scan_columns(n, rng)
     devs = [Dev(c) for c in cols]

@@ -1,15 +1,10 @@
 """The ranked-bitmap lookup of the fused star pipeline (b2_star_build_mark / _rank / _fill, probed by
 b2_star_agg): dimension shapes that exercise the directory's rank and the slot array, against pandas."""
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pandas as pd
 import pytest
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 RTOL = 1e-9
 
 
@@ -106,17 +101,3 @@ def test_star_bitmap_lookup_twice_on_prepared_plan():
         np.testing.assert_array_equal(got["grp"].to_numpy(), exp["grp"].to_numpy())
         np.testing.assert_array_equal(got["n"].to_numpy(), exp["n"].to_numpy())
         np.testing.assert_allclose(got["rev"].to_numpy(), exp["rev"].to_numpy(), rtol=RTOL)
-
-
-def test_star_bitmap_lookup_staged_pipeline():
-    """The same cases through the TMA-staged instance of b2_star_agg (B200SQL_PIPELINE=1, read once
-    per process): in a child process."""
-    if os.environ.get("B200SQL_PIPELINE") == "1":
-        pytest.skip("already the staged instance")
-    env = dict(os.environ, B200SQL_PIPELINE="1")
-    res = subprocess.run(
-        [sys.executable, "-m", "pytest", "tests/test_gpu_star_bitmap.py", "-m", "gpu", "-x", "-q", "-k",
-         "not staged_pipeline"],
-        cwd=ROOT, env=env, capture_output=True, text=True, timeout=600)
-    assert res.returncode == 0, res.stdout[-3000:] + res.stderr[-2000:]
-    assert " passed" in res.stdout

@@ -2,11 +2,8 @@
 21 and 32 bits: b2_star_build_fill_packed word for word against tests/star_packed_ref.py, then b2_star_agg
 probing it (per-row slots and aggregates against the reference), with null_slot at and next to each width's
 edge.  Then end-to-end SQL in the C4 shape with group-key ranges that select each width, through a prepared
-plan whose lookup buffer holds garbage before its second run, and through the TMA-staged instance."""
+plan whose lookup buffer holds garbage before its second run."""
 import ctypes as C
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pandas as pd
@@ -20,7 +17,6 @@ from tests.test_gpu_groupagg import (COUNT, DIM_PRED, GRP_MIN, PRED, SUM, AMAX, 
                                      fact_part, scan_of)
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 # (null_slot, width): at and next to each class edge
 EDGES = [(2 ** 16 - 2, 16), (2 ** 16 - 1, 16), (2 ** 16, 21), (2 ** 21 - 1, 21), (2 ** 21, 32), (2 ** 21 + 1, 32)]
@@ -285,17 +281,3 @@ def test_c4_shape_unprepared(ng, bits, monkeypatch):
     got, nothing_cached, _ = run(q.format(" * 2"))
     _check(got.assign(rev=got["rev"] / 2), exp)
     assert nothing_cached
-
-
-def test_packed_staged_pipeline():
-    """Everything above through the TMA-staged instance of b2_star_agg (B200SQL_PIPELINE=1, read once per
-    process): in a child process."""
-    if os.environ.get("B200SQL_PIPELINE") == "1":
-        pytest.skip("already the staged instance")
-    env = dict(os.environ, B200SQL_PIPELINE="1")
-    res = subprocess.run(
-        [sys.executable, "-m", "pytest", "tests/test_gpu_star_packed.py", "-m", "gpu", "-x", "-q", "-k",
-         "not staged_pipeline"],
-        cwd=ROOT, env=env, capture_output=True, text=True, timeout=900)
-    assert res.returncode == 0, res.stdout[-3000:] + res.stderr[-2000:]
-    assert " passed" in res.stdout
