@@ -185,7 +185,7 @@ b2_part_scatter_kernel(const __grid_constant__ b2_scan_t s, int key_col, int64_t
       if (slot[j] >= 0) {
         const int b = (int)(slot[j] >> shift);
         const int p = prefix[b] + rank[j];
-        st_key[p] = kmin + slot[j];
+        st_key[p] = (int64_t)((uint64_t)kmin + (uint64_t)slot[j]);   // wraps: the NULL slot may lie past INT64_MAX
         st_src[p] = (uint16_t)(local0 + j * 32);
         st_bkt[p] = (uint16_t)b;
       }

@@ -1094,7 +1094,8 @@ def grouped_aggregate(parts, pred, gexprs, gnames, plan: AggPlan, child, sharded
             stats["launches"] += 1
             L.range_partition_scan(nbuckets, D.ptr(ws), D.stream_ptr())
             ctx0 = work[0][1]
-            out_key = torch.full((n_all,), kmin + nslots + 1, dtype=torch.int64, device=dev)
+            # rows no bucket claims keep a key whose slot, nslots + 1, is past the table (wrapping like the kernels)
+            out_key = torch.full((n_all,), _wrap64(kmin + nslots + 1), dtype=torch.int64, device=dev)
             outs = [torch.empty(n_all, dtype=_TORCH_DT[ctx0.cols[c].dtype], device=dev) for c in carried]
             cc = (C.c_int32 * max(1, len(carried)))(*carried)
             oc = (C.c_void_p * max(1, len(carried)))(*[o.data_ptr() for o in outs])
@@ -1417,6 +1418,19 @@ def _gather_view(view: SlotView, idx, dev):
 DEFER_MAX_SLOTS = 1 << 23    # deferred compaction allocates its outputs at one row per slot of the window
 
 
+def _wrap64(x: int) -> int:
+    """x reduced to the int64 range (two's complement), as the kernels' uint64 slot arithmetic sees it"""
+    return (x + (1 << 63)) % (1 << 64) - (1 << 63)
+
+
+def _slot_keys(kmin, lo, count, dev) -> torch.Tensor:
+    """int64 group key of each slot of the window [lo, lo + count): kmin + slot, wrapping.  A key range
+    that ends at INT64_MAX puts the NULL slot (and a padded slice's tail) past it; those keys are never
+    read as values, but torch.arange(kmin + lo, kmin + lo + count) would refuse the end."""
+    keys = torch.arange(count, dtype=torch.int64, device=dev)
+    return keys.add_(_wrap64(kmin + lo))
+
+
 def _finalize_dense(view: SlotView, kmin, gname, gexpr, glog, plan, dev, key_nullable=True,
                     check=None, fallback=None) -> Part:
     """Window of a dense table -> result partition (group key = kmin + slot; the table's last slot
@@ -1429,7 +1443,7 @@ def _finalize_dense(view: SlotView, kmin, gname, gexpr, glog, plan, dev, key_nul
     if not key_nullable and gexpr.dtype == I64 and count <= DEFER_MAX_SLOTS and ncols <= L.MAX_GATHER \
             and os.environ.get("B200SQL_NO_DEFER") != "1":
         with _Phase("compact"):
-            slot_keys = torch.arange(kmin + view.lo, kmin + view.lo + count, dtype=torch.int64, device=dev)
+            slot_keys = _slot_keys(kmin, view.lo, count, dev)
             occ, term = view.occupancy(slot_keys)
             cols, where = [occ, DeviceColumn(slot_keys, None, I64)], {}
             for i, (acc, cnt) in enumerate(zip(view.acc, view.cnt)):
@@ -1475,7 +1489,7 @@ def _finalize_dense(view: SlotView, kmin, gname, gexpr, glog, plan, dev, key_nul
 
 def _extract_dense(view: SlotView, kmin, gname, gexpr, glog, dev, key_nullable=True) -> RawGroups:
     count = view.count
-    slot_keys = torch.arange(kmin + view.lo, kmin + view.lo + count, dtype=torch.int64, device=dev)
+    slot_keys = _slot_keys(kmin, view.lo, count, dev)
     occ, term = view.occupancy(slot_keys)
     if not key_nullable and gexpr.dtype == I64:
         # the key column has no NULLs, so the NULL slot stays empty: no validity work.

@@ -23,8 +23,9 @@ from typing import Optional
 
 from .... import config as dask_config
 from ....datacontainer import ColumnContainer, DataContainer
-from ....frame import AggSource, LazyFrame, LazySeries
-from ....expr import ColRef
+from ....frame import AggSource, LazyFrame, LazySeries, TableSource
+from .... import expr as E
+from ....expr import F64, I64, U8, Call, ColRef, Lit
 from ....utils import new_temporary_column
 from ...rex.convert import RexConverter
 from ..base import BaseRelPlugin
@@ -127,6 +128,39 @@ class DaskAggregatePlugin(BaseRelPlugin):
         name = new_temporary_column(frame)
         return frame.assign(**{name: series}), name
 
+    @staticmethod
+    def _null_safe_keys(frame: LazyFrame, keys, nullable, tag):
+        """(frame, join columns) on which the groups of two passes over the same input meet, the NULL group
+        included.  An equi-join never matches NULL keys, which would leave the DISTINCT aggregates of the NULL
+        group NULL; so a key that may be NULL (or a NaN float) joins on its value with NULL replaced by zero,
+        and one more column holds the NULL flags of all such keys as a bitmask.  A key that is never NULL
+        joins as it is (k such keys: the same k-column join as before, dense when it can be).  A VARCHAR key
+        joins on its dictionary codes: both passes read the same column, so one dictionary."""
+        exprs, names, mask = OrderedDict(frame.exprs), [], None
+        for i, (k, nul) in enumerate(zip(keys, nullable)):
+            if not nul:
+                names.append(k)
+                continue
+            e = frame.exprs[k]
+            null = Call("isnull", [e], U8)
+            exprs[f"{tag}v{i}"] = Call("case", [null, Lit(0.0 if e.dtype == F64 else 0, e.dtype), e], e.dtype)
+            names.append(f"{tag}v{i}")
+            bit = E.binop("mul", E.cast(null, I64), 1 << i)
+            mask = bit if mask is None else E.binop("add", mask, bit)
+        if mask is not None:
+            exprs[f"{tag}m"] = mask
+            names.append(f"{tag}m")
+        return LazyFrame(frame.source, exprs, frame.pred), names
+
+    @staticmethod
+    def _key_nullable(frame: LazyFrame, k) -> bool:
+        """can group key k of the input be NULL, or a NaN (a NULL float key)?"""
+        e = frame.exprs[k]
+        if e.dtype == F64:
+            return True
+        table = frame.source.table if isinstance(frame.source, TableSource) else None
+        return E.may_be_null(e, (lambda n: table.column_nullable(n)) if table is not None else (lambda n: True))
+
     def _run_passes(self, frame, keys, calls, options):
         shared, per_distinct_input = [], OrderedDict()
         for c in calls:
@@ -162,6 +196,7 @@ class DaskAggregatePlugin(BaseRelPlugin):
             one = new_temporary_column(frame)
             passes = [(f.assign(**{one: 0}), specs) for f, specs in passes]
             join_keys = [one]
+        nullable = [k in keys and self._key_nullable(frame, k) for k in join_keys]
         result = None
         for source, specs in passes:
             part = LazyFrame(AggSource(source, join_keys, specs, options))
@@ -169,8 +204,12 @@ class DaskAggregatePlugin(BaseRelPlugin):
                 result = part
                 continue
             # the first pass holds every group (it saw every row); later ones hang off it
-            theirs = {k: f"{k}__pass{len(result.columns)}" for k in join_keys}
-            merged = result.merge(part.rename(theirs), how="left", left_on=join_keys,
-                                  right_on=[theirs[k] for k in join_keys])
+            tag = len(result.columns)
+            mine, on_mine = self._null_safe_keys(result, join_keys, nullable, f"__l{tag}")
+            theirs, on_theirs = self._null_safe_keys(part, join_keys, nullable, f"__r{tag}")
+            theirs = theirs.rename({k: f"{k}__pass{tag}" for k in join_keys if k in on_theirs})
+            on_theirs = [f"{k}__pass{tag}" if k in join_keys else k for k in on_theirs]
+            merged = mine.merge(theirs[on_theirs + [out for _, out, _ in specs]], how="left",
+                                left_on=on_mine, right_on=on_theirs)
             result = merged[list(result.columns) + [out for _, out, _ in specs]]
         return result if join_keys is keys else result[[c for c in result.columns if c not in join_keys]]

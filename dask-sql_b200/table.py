@@ -206,7 +206,7 @@ def _host_column(values, pin=True) -> HostColumn:
     elif isinstance(values, pd.Series):
         arr = values.array
         if isinstance(arr, pd.arrays.BooleanArray):
-            mask, vals = np.asarray(arr._mask), np.asarray(arr._data).astype(np.uint8)
+            mask, vals = np.asarray(arr._mask), np.asarray(arr._data)     # bool: stays a U8 column
         elif isinstance(arr, (pd.arrays.IntegerArray, pd.arrays.FloatingArray)):
             mask, vals = np.asarray(arr._mask), np.asarray(arr._data)
         else:
