@@ -11,7 +11,7 @@ LIB_PATH = os.environ.get("B200SQL_LIB") or os.path.join(HERE, "libb200sql.so") 
 
 # ---- constants (mirror include/b200sql.h) ----
 I64, F64, U8 = 0, 1, 2
-U32 = 3          # storage-only: narrowed key-ordered join payload
+U32 = 3          # storage-only: narrowed key-ordered join payload, or a star scan's image of an int64 column
 COL_SENTINEL = 1
 MAX_COLS, MAX_TERMS, MAX_AGGS, MAX_KEYS, MAX_GATHER, MAX_PROG = 16, 8, 8, 4, 8, 64
 TILE = 4096
@@ -198,6 +198,7 @@ _SIGS = {
     "b2_peer_merge": [C.POINTER(PeerMerge), _P],
     "b2_sort_by": [C.POINTER(Col), C.c_int64, C.c_int32, C.c_int32, _P, _P, _P],
     "b2_dense_slots": [C.POINTER(Col), C.c_int64, C.c_int64, C.c_int32, _P, _P],
+    "b2_narrow_image": [C.POINTER(Col), C.c_int64, C.c_int64, _P, _P],
     "b2_star_build_dense": [C.POINTER(Col), _P, C.c_int64, _P, C.c_int64, C.c_int64, _P, _P, _P],
     "b2_star_build_mark": [C.POINTER(Scan), C.c_int32, C.c_int64, C.c_int64, _P, _P, _P],
     "b2_star_build_rank": [_P, C.c_int64, _P],
@@ -208,6 +209,11 @@ _SIGS = {
     "b2_star_build_hash": [C.POINTER(Col), _P, C.c_int64, _P, _P, _P, C.c_int64, _P, _P],
     "b2_star_agg": [C.POINTER(Scan), C.c_int32, C.POINTER(StarLookup), C.POINTER(Agg), C.c_int32,
                     C.POINTER(AggState), _P],
+    "b2_star_build_mark_narrow": [C.POINTER(Scan), _P, C.c_int32, C.c_int64, C.c_int64, _P, _P, _P],
+    "b2_star_build_fill_narrow": [C.POINTER(Scan), _P, C.c_int32, C.c_int32, C.c_int64, C.c_int64, C.c_int64,
+                                  C.c_int32, _P, _P, C.c_int32, _P],
+    "b2_star_agg_narrow": [C.POINTER(Scan), _P, C.c_int32, C.POINTER(StarLookup), C.POINTER(Agg), C.c_int32,
+                           C.POINTER(AggState), _P],
     "b2_str_like": [_P, _P, C.c_int64, _P, C.c_int64, C.c_uint32, C.c_int32, _P, _P],
     "b2_str_lower_bound": [_P, _P, C.c_int64, _P, _P, C.c_int64, C.c_int32, _P, _P, _P],
 }
@@ -293,6 +299,7 @@ _lib.b2_sort_ws_bytes.restype = C.c_int64
 _lib.b2_sort_ws_bytes.argtypes = [C.c_int64]
 sort_ws_bytes = _lib.b2_sort_ws_bytes
 dense_slots = _wrap("b2_dense_slots")
+narrow_image = _wrap("b2_narrow_image")
 star_build_dense = _wrap("b2_star_build_dense")
 star_build_mark = _wrap("b2_star_build_mark")
 star_build_rank = _wrap("b2_star_build_rank")
@@ -300,6 +307,9 @@ star_build_fill = _wrap("b2_star_build_fill")
 star_build_fill_packed = _wrap("b2_star_build_fill_packed")
 star_build_hash = _wrap("b2_star_build_hash")
 star_agg = _wrap("b2_star_agg")
+star_build_mark_narrow = _wrap("b2_star_build_mark_narrow")
+star_build_fill_narrow = _wrap("b2_star_build_fill_narrow")
+star_agg_narrow = _wrap("b2_star_agg_narrow")
 str_like = _wrap("b2_str_like")
 str_lower_bound = _wrap("b2_str_lower_bound")
 num_tiles = _lib.b2_num_tiles

@@ -140,6 +140,11 @@ __device__ __forceinline__ int64_t b2_ld_stream(const int64_t* p) {
   asm("ld.global.nc.L2::cache_hint.b64 %0, [%1], %2;" : "=l"(v) : "l"(p), "l"(b2_policy_stream()));
   return v;
 }
+__device__ __forceinline__ uint32_t b2_ld_stream_u32(const uint32_t* p) {
+  uint32_t v;
+  asm("ld.global.nc.L2::cache_hint.b32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(b2_policy_stream()));
+  return v;
+}
 // table load that should stay in L2
 __device__ __forceinline__ int32_t b2_ld_keep_i32(const int32_t* p) {
   int32_t v;
@@ -244,12 +249,35 @@ __device__ __forceinline__ void b2_load_batch8(const void* data, int64_t row0, u
 #pragma unroll
   for (int j = 0; j < R; ++j) raw[j] = (full || ((bits >> j) & 1)) ? (int64_t)p[j * 32] : 0;
 }
+// R values of a B2_U32 image (b2_narrow_image): 4 bytes per row, widened as an unsigned add so that an image
+// whose range touches INT64_MIN or INT64_MAX comes back exact.  Only the loader of the star kernels
+// (b2_gld_t<true>) calls it, so that no other kernel carries the third branch.
 template <int R>
+__device__ __forceinline__ void b2_load_batch32(const void* data, int64_t base, int64_t row0, uint32_t bits, bool full,
+                                                int64_t (&raw)[R]) {
+  const uint32_t* p = reinterpret_cast<const uint32_t*>(data) + row0;
+#pragma unroll
+  for (int j = 0; j < R; ++j) {
+    const uint32_t off = (full || ((bits >> j) & 1)) ? b2_ld_stream_u32(p + j * 32) : 0u;
+    raw[j] = (int64_t)((uint64_t)base + off);
+  }
+}
+// base: where a B2_U32 column's base is (NARROW instances only)
+template <int R, bool NARROW = false>
 __device__ __forceinline__ void b2_load_batch(const b2_col_t& c, int64_t row0, uint32_t bits, bool full,
-                                              int64_t (&raw)[R]) {
+                                              int64_t (&raw)[R], const int64_t* base = nullptr) {
   if (c.dtype == B2_U8) b2_load_batch8<R>(c.data, row0, bits, full, raw);
+  else if (NARROW && c.dtype == B2_U32) b2_load_batch32<R>(c.data, *base, row0, bits, full, raw);
   else b2_load_batch64<R>(c.data, row0, bits, full, raw);
 }
+
+// the parameter of the star kernels: a scan and the bases of its B2_U32 image columns (b2_star_*_narrow), read
+// from the constant bank like the column descriptors.  The loader reaches base[] from the address of `s`, the
+// first member, so that no second pointer stays live in a kernel that has no register to spare.
+struct b2_scan_narrow_t {
+  b2_scan_t s;
+  int64_t base[B2_MAX_COLS];
+};
 
 // validity bits of the batch (bit j = row j valid).  Bitmap bytes: row0+32j -> byte (row0>>3)+4j
 template <int R>
@@ -319,22 +347,25 @@ __device__ __forceinline__ uint32_t b2_cmp_batch_f(const int64_t (&raw)[R], doub
 // ---------------------------------------------------------------------------------------
 // column loader and the tile loops that hand it to a batch body
 // ---------------------------------------------------------------------------------------
-struct b2_gld {  // straight from global memory
+template <bool NARROW>   // NARROW: s is the .s of a b2_scan_narrow_t and may hold B2_U32 images
+struct b2_gld_t {  // straight from global memory
   const b2_scan_t* s;
   int64_t row0;
   template <int R>
   __device__ __forceinline__ void load(int col, uint32_t bits, bool full, int64_t (&raw)[R]) const {
-    b2_load_batch<R>(s->cols[col], row0, bits, full, raw);
+    b2_load_batch<R, NARROW>(s->cols[col], row0, bits, full, raw,
+                             NARROW ? reinterpret_cast<const b2_scan_narrow_t*>(s)->base + col : nullptr);
   }
 };
+using b2_gld = b2_gld_t<false>;
 
 // body(ld) once per tile of B2_BLOCK x R rows, tiles grid-strided over the CTAs
-template <int R, class Body>
+template <int R, bool NARROW = false, class Body>
 __device__ __forceinline__ void b2_tile_direct(const b2_scan_t& s, Body&& body) {
   const int tile_off = (threadIdx.x >> 5) * (32 * R) + (threadIdx.x & 31);
   const int64_t tile = (int64_t)B2_BLOCK * R;
   for (int64_t base = (int64_t)blockIdx.x * tile; base < s.n; base += (int64_t)gridDim.x * tile) {
-    const b2_gld ld{&s, base + tile_off};
+    const b2_gld_t<NARROW> ld{&s, base + tile_off};
     body(ld);
   }
 }
@@ -363,8 +394,8 @@ __device__ __forceinline__ void b2_tile_ticket(const b2_scan_t& s, unsigned long
 
 // Evaluate all predicate terms for the batch.  Returns the surviving row bits and whether the
 // batch is fully in bounds.
-template <int R>
-__device__ __forceinline__ uint32_t b2_eval_terms(const b2_scan_t& s, const b2_gld& ld, bool& full, int& last_col,
+template <int R, bool N>
+__device__ __forceinline__ uint32_t b2_eval_terms(const b2_scan_t& s, const b2_gld_t<N>& ld, bool& full, int& last_col,
                                                   int64_t (&raw)[R]) {
   // On return `raw` still holds the values of column `last_col` (the last term's column, -1 if
   // none) for the surviving rows: consumers that need the same column again (SUM(x) ... WHERE x > 0,
@@ -399,8 +430,8 @@ __device__ __forceinline__ uint32_t b2_eval_terms(const b2_scan_t& s, const b2_g
   }
   return bits;
 }
-template <int R>
-__device__ __forceinline__ uint32_t b2_eval_terms(const b2_scan_t& s, const b2_gld& ld, bool& full) {
+template <int R, bool N>
+__device__ __forceinline__ uint32_t b2_eval_terms(const b2_scan_t& s, const b2_gld_t<N>& ld, bool& full) {
   int last_col;
   int64_t raw[R];
   return b2_eval_terms<R>(s, ld, full, last_col, raw);
@@ -492,8 +523,8 @@ struct b2_aggs_arg {  // aggs passed by value in kernel params
 // load its input column for the contributing rows, drop NULLs, apply the atomics.
 // `pre` (optional): values of aggregate 0's input column already loaded by the caller for the rows
 // in `pre_bits` (a superset of the contributing rows), so that this load overlapped the slot lookup.
-template <int R>
-__device__ __forceinline__ void b2_apply_aggs(const b2_scan_t& s, const b2_gld& ld, const b2_agg_t* __restrict__ aggs,
+template <int R, bool N>
+__device__ __forceinline__ void b2_apply_aggs(const b2_scan_t& s, const b2_gld_t<N>& ld, const b2_agg_t* __restrict__ aggs,
                                               int naggs, const b2_aggstate_t& st,
                                               const int64_t (&slot)[R], const int64_t* pre = nullptr) {
   const int64_t row0 = ld.row0;

@@ -373,9 +373,13 @@ extern "C" {
 
 int64_t b2_scan_agg_ws_bytes(void) { return (int64_t)sizeof(b2_partial) * B2_MAX_PARTIALS; }
 
-static int32_t b2_check_scan(const b2_scan_t* s) {
+// narrow: the entry point reads its scan columns only through b2_load_batch, which widens B2_U32 images
+// (b2_narrow_image); every other one reads c.data as 1 or 8 bytes per row and must never see one
+static int32_t b2_check_scan(const b2_scan_t* s, bool narrow = false) {
   B2_REQUIRE(s, "null scan");
   B2_REQUIRE(s->ncols >= 0 && s->ncols <= B2_MAX_COLS, "bad ncols");
+  for (int c = 0; c < s->ncols; ++c)
+    B2_REQUIRE(narrow || s->cols[c].dtype != B2_U32, "a B2_U32 image column is only read by the star scans");
   B2_REQUIRE(s->nterms >= 0 && s->nterms <= B2_MAX_TERMS, "bad nterms");
   B2_REQUIRE(s->n >= 0 && s->n < ((int64_t)1 << 31), "partition must hold < 2^31 rows");
   for (int t = 0; t < s->nterms; ++t) {

@@ -240,6 +240,14 @@ b2_dense_slots_kernel(const __grid_constant__ b2_col_t key, int64_t n, int64_t k
   }
 }
 
+// the 32-bit image that the star scans stream in place of an int64 column (include/b200sql.h, b2_narrow_image)
+__global__ void __launch_bounds__(B2_BLOCK)
+b2_narrow_image_kernel(const int64_t* __restrict__ data, const uint8_t* __restrict__ valid, int64_t n, int64_t base,
+                       uint32_t* __restrict__ out) {
+  for (int64_t i = (int64_t)blockIdx.x * B2_BLOCK + threadIdx.x; i < n; i += (int64_t)gridDim.x * B2_BLOCK)
+    out[i] = (valid && !b2_bit(valid, i)) ? 0u : (uint32_t)((uint64_t)data[i] - (uint64_t)base);
+}
+
 __global__ void __launch_bounds__(B2_BLOCK)
 b2_star_build_dense_kernel(const __grid_constant__ b2_col_t pk, const int32_t* __restrict__ sel, int64_t n_sel,
                            const int32_t* __restrict__ slot_of_row, int64_t kmin, int64_t range,
@@ -273,15 +281,16 @@ __device__ __forceinline__ uint32_t b2_slot_word(uint32_t pos, int slot_bits) {
 
 template <bool FILL>
 __global__ void __launch_bounds__(B2_BLOCK)
-b2_star_build_scan_kernel(const __grid_constant__ b2_scan_t s, int pk_col, int grp_col, int64_t pk_min,
+b2_star_build_scan_kernel(const __grid_constant__ b2_scan_narrow_t sn, int pk_col, int grp_col, int64_t pk_min,
                           int64_t pk_range, int64_t grp_min, int32_t null_slot, uint64_t* __restrict__ dir,
                           void* __restrict__ slots, int slot_bits, int32_t* __restrict__ flags) {
+  const b2_scan_t& s = sn.s;
   const int tile_off = (threadIdx.x >> 5) * (32 * B2_GB_R) + (threadIdx.x & 31);
   const b2_col_t& pc = s.cols[pk_col];
   const b2_col_t& gc = s.cols[grp_col];
   for (int64_t base = (int64_t)blockIdx.x * B2_GB_ROWS_PER_BLOCK; base < s.n;
        base += (int64_t)gridDim.x * B2_GB_ROWS_PER_BLOCK) {
-    const b2_gld ld{&s, base + tile_off};
+    const b2_gld_t<true> ld{&s, base + tile_off};
     bool full;
     const uint32_t bits = b2_eval_terms<B2_GB_R>(s, ld, full);
     int64_t pk[B2_GB_R];
@@ -469,7 +478,7 @@ __device__ __forceinline__ int32_t b2_star_lookup(const b2_starlookup_t& lk, int
 // more independent loads in flight per thread.
 #define B2_STAR_R 16
 template <int R>
-__device__ __forceinline__ void b2_star_body(const b2_scan_t& s, const b2_gld& ld, int fk_col, const b2_starlookup_t& lk,
+__device__ __forceinline__ void b2_star_body(const b2_scan_t& s, const b2_gld_t<true>& ld, int fk_col, const b2_starlookup_t& lk,
                                              const b2_aggs_arg& aggs, const b2_aggstate_t& st) {
   // Two memory round trips per batch instead of four:
   //   1. the join-key column is requested together with the predicate columns (its sectors are
@@ -557,9 +566,10 @@ __device__ __forceinline__ void b2_star_body(const b2_scan_t& s, const b2_gld& l
 }
 
 __global__ void __launch_bounds__(B2_BLOCK)
-b2_star_agg_kernel(const __grid_constant__ b2_scan_t s, int fk_col, const __grid_constant__ b2_starlookup_t lk,
+b2_star_agg_kernel(const __grid_constant__ b2_scan_narrow_t sn, int fk_col, const __grid_constant__ b2_starlookup_t lk,
                    const __grid_constant__ b2_aggs_arg aggs, const __grid_constant__ b2_aggstate_t st) {
-  b2_tile_direct<B2_STAR_R>(s, [&](const b2_gld& ld) { b2_star_body<B2_STAR_R>(s, ld, fk_col, lk, aggs, st); });
+  const b2_scan_t& s = sn.s;
+  b2_tile_direct<B2_STAR_R, true>(s, [&](const b2_gld_t<true>& ld) { b2_star_body<B2_STAR_R>(s, ld, fk_col, lk, aggs, st); });
 }
 
 extern "C" {
@@ -574,6 +584,19 @@ static int32_t b2_check_state(const b2_aggs_arg& aa, const b2_aggstate_t* st) {
   return B2_OK;
 }
 static inline bool b2_pow2(int64_t x) { return x > 0 && (x & (x - 1)) == 0; }
+// an int64 column, or its B2_U32 image, which the star scans widen back to int64 as they load it
+static inline bool b2_is_int64_scan_col(const b2_col_t& c) { return c.dtype == B2_I64 || c.dtype == B2_U32; }
+// the scan check of the star entry points (B2_U32 image columns only with their bases; NULL: none) and their
+// kernel parameter
+static int32_t b2_check_narrow_scan(const b2_scan_t* scan, const int64_t* bases, b2_scan_narrow_t* out) {
+  int32_t rc = b2_check_scan(scan, bases != nullptr);
+  if (rc) return rc;
+  memset(out, 0, sizeof(*out));
+  out->s = *scan;
+  if (bases)
+    for (int c = 0; c < scan->ncols; ++c) out->base[c] = bases[c];
+  return B2_OK;
+}
 
 static int32_t b2_groupby_dense_impl(const b2_scan_t* scan, int32_t key_col, int64_t kmin, int64_t nslots,
                                      const b2_agg_t* aggs, int32_t naggs, const b2_aggstate_t* st,
@@ -733,6 +756,17 @@ int32_t b2_dense_slots(const b2_col_t* key, int64_t n, int64_t kmin, int32_t nul
   return B2_OK;
 }
 
+int32_t b2_narrow_image(const b2_col_t* col, int64_t n, int64_t base, uint32_t* out, void* stream) {
+  B2_REQUIRE(col && out, "null argument");
+  B2_REQUIRE(col->dtype == B2_I64, "an image is made of an int64 column");
+  if (n <= 0) return B2_OK;
+  int grid = b2_wave_grid(b2_narrow_image_kernel, B2_BLOCK, (n + B2_BLOCK - 1) / B2_BLOCK);
+  b2_narrow_image_kernel<<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(static_cast<const int64_t*>(col->data), col->valid,
+                                                                       n, base, out);
+  B2_CHECK_LAUNCH("b2_narrow_image_kernel");
+  return B2_OK;
+}
+
 int32_t b2_star_build_dense(const b2_col_t* pk, const int32_t* sel, int64_t n_sel, const int32_t* slot_of_row,
                             int64_t kmin, int64_t range, int32_t* lookup, int32_t* d_flags, void* stream) {
   B2_REQUIRE(pk && slot_of_row && lookup && d_flags, "null argument");
@@ -745,33 +779,42 @@ int32_t b2_star_build_dense(const b2_col_t* pk, const int32_t* sel, int64_t n_se
   return B2_OK;
 }
 
-static int32_t b2_star_build_pass(bool fill, const b2_scan_t* scan, int32_t pk_col, int32_t grp_col,
-                                  int64_t pk_min, int64_t pk_range, int64_t grp_min, int32_t null_slot,
-                                  uint64_t* dir, void* slots, int32_t slot_bits, int32_t* d_flags, void* stream) {
-  int32_t rc = b2_check_scan(scan);
+static int32_t b2_star_build_pass(bool fill, const b2_scan_t* scan, const int64_t* bases, int32_t pk_col,
+                                  int32_t grp_col, int64_t pk_min, int64_t pk_range, int64_t grp_min,
+                                  int32_t null_slot, uint64_t* dir, void* slots, int32_t slot_bits, int32_t* d_flags,
+                                  void* stream) {
+  b2_scan_narrow_t sn;
+  int32_t rc = b2_check_narrow_scan(scan, bases, &sn);
   if (rc) return rc;
   B2_REQUIRE(pk_col >= 0 && pk_col < scan->ncols && grp_col >= 0 && grp_col < scan->ncols, "column out of range");
-  B2_REQUIRE(scan->cols[pk_col].dtype == B2_I64 && scan->cols[grp_col].dtype == B2_I64, "dense keys must be int64");
+  B2_REQUIRE(b2_is_int64_scan_col(scan->cols[pk_col]) && b2_is_int64_scan_col(scan->cols[grp_col]),
+             "dense keys must be int64");
   B2_REQUIRE(pk_range > 0 && pk_range < ((int64_t)1 << 31), "bad range");
   if (scan->n == 0) return B2_OK;
   int64_t nblk = (scan->n + B2_GB_ROWS_PER_BLOCK - 1) / B2_GB_ROWS_PER_BLOCK;
   if (fill) {
     int grid = b2_wave_grid(b2_star_build_scan_kernel<true>, B2_BLOCK, nblk);
-    b2_star_build_scan_kernel<true><<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(*scan, pk_col, grp_col, pk_min, pk_range,
+    b2_star_build_scan_kernel<true><<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(sn, pk_col, grp_col, pk_min, pk_range,
                                                                                   grp_min, null_slot, dir, slots, slot_bits, d_flags);
   } else {
     int grid = b2_wave_grid(b2_star_build_scan_kernel<false>, B2_BLOCK, nblk);
-    b2_star_build_scan_kernel<false><<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(*scan, pk_col, grp_col, pk_min, pk_range,
+    b2_star_build_scan_kernel<false><<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(sn, pk_col, grp_col, pk_min, pk_range,
                                                                                    grp_min, null_slot, dir, slots, slot_bits, d_flags);
   }
   B2_CHECK_LAUNCH("b2_star_build_scan_kernel");
   return B2_OK;
 }
 
+int32_t b2_star_build_mark_narrow(const b2_scan_t* scan, const int64_t* bases, int32_t pk_col, int64_t pk_min,
+                                  int64_t pk_range, uint64_t* dir, int32_t* d_flags, void* stream) {
+  B2_REQUIRE(dir && d_flags, "null argument");
+  return b2_star_build_pass(false, scan, bases, pk_col, pk_col, pk_min, pk_range, 0, 0, dir, nullptr, 32, d_flags,
+                            stream);
+}
+
 int32_t b2_star_build_mark(const b2_scan_t* scan, int32_t pk_col, int64_t pk_min, int64_t pk_range, uint64_t* dir,
                            int32_t* d_flags, void* stream) {
-  B2_REQUIRE(dir && d_flags, "null argument");
-  return b2_star_build_pass(false, scan, pk_col, pk_col, pk_min, pk_range, 0, 0, dir, nullptr, 32, d_flags, stream);
+  return b2_star_build_mark_narrow(scan, nullptr, pk_col, pk_min, pk_range, dir, d_flags, stream);
 }
 
 int32_t b2_star_build_rank(uint64_t* dir, int64_t pk_range, void* stream) {
@@ -798,11 +841,18 @@ int32_t b2_star_build_fill(const b2_scan_t* scan, int32_t pk_col, int32_t grp_co
 int32_t b2_star_build_fill_packed(const b2_scan_t* scan, int32_t pk_col, int32_t grp_col, int64_t pk_min,
                                   int64_t pk_range, int64_t grp_min, int32_t null_slot, const uint64_t* dir,
                                   uint64_t* slots, int32_t slot_bits, void* stream) {
+  return b2_star_build_fill_narrow(scan, nullptr, pk_col, grp_col, pk_min, pk_range, grp_min, null_slot, dir, slots,
+                                   slot_bits, stream);
+}
+
+int32_t b2_star_build_fill_narrow(const b2_scan_t* scan, const int64_t* bases, int32_t pk_col, int32_t grp_col,
+                                  int64_t pk_min, int64_t pk_range, int64_t grp_min, int32_t null_slot,
+                                  const uint64_t* dir, uint64_t* slots, int32_t slot_bits, void* stream) {
   B2_REQUIRE(dir && slots, "null argument");
   B2_REQUIRE(slot_bits == 16 || slot_bits == 21 || slot_bits == 32, "slot_bits must be 16, 21 or 32");
   B2_REQUIRE(slot_bits == 32 || (null_slot >= 0 && null_slot < (1 << slot_bits)), "null_slot does not fit slot_bits");
   B2_REQUIRE(slot_bits == 32 || ((uintptr_t)slots & 7) == 0, "packed slots must be 8-byte aligned");
-  return b2_star_build_pass(true, scan, pk_col, grp_col, pk_min, pk_range, grp_min, null_slot,
+  return b2_star_build_pass(true, scan, bases, pk_col, grp_col, pk_min, pk_range, grp_min, null_slot,
                             const_cast<uint64_t*>(dir), slots, slot_bits, nullptr, stream);
 }
 
@@ -822,14 +872,20 @@ int32_t b2_star_build_hash(const b2_col_t* pk, const int32_t* sel, int64_t n_sel
 
 int32_t b2_star_agg(const b2_scan_t* scan, int32_t fk_col, const b2_starlookup_t* lk, const b2_agg_t* aggs,
                     int32_t naggs, const b2_aggstate_t* st, void* stream) {
-  int32_t rc = b2_check_scan(scan);
+  return b2_star_agg_narrow(scan, nullptr, fk_col, lk, aggs, naggs, st, stream);
+}
+
+int32_t b2_star_agg_narrow(const b2_scan_t* scan, const int64_t* bases, int32_t fk_col, const b2_starlookup_t* lk,
+                           const b2_agg_t* aggs, int32_t naggs, const b2_aggstate_t* st, void* stream) {
+  b2_scan_narrow_t sn;
+  int32_t rc = b2_check_narrow_scan(scan, bases, &sn);
   if (rc) return rc;
   b2_aggs_arg aa;
   if ((rc = b2_check_aggs(scan, aggs, naggs, &aa))) return rc;
   if ((rc = b2_check_state(aa, st))) return rc;
   B2_REQUIRE(lk, "null lookup");
   B2_REQUIRE(fk_col >= 0 && fk_col < scan->ncols, "fk column out of range");
-  B2_REQUIRE(scan->cols[fk_col].dtype == B2_I64, "fk must be int64");
+  B2_REQUIRE(b2_is_int64_scan_col(scan->cols[fk_col]), "fk must be int64");
   B2_REQUIRE(lk->dense >= 0 && lk->dense <= 2, "bad lookup kind");
   b2_starlookup_t l = *lk;
   if (l.dense == 2) {
@@ -843,7 +899,7 @@ int32_t b2_star_agg(const b2_scan_t* scan, int32_t fk_col, const b2_starlookup_t
   if (scan->n == 0) return B2_OK;
   int64_t nblk = (scan->n + (int64_t)B2_BLOCK * B2_STAR_R - 1) / ((int64_t)B2_BLOCK * B2_STAR_R);
   int grid = b2_wave_grid(b2_star_agg_kernel, B2_BLOCK, nblk);
-  b2_star_agg_kernel<<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(*scan, fk_col, l, aa, *st);
+  b2_star_agg_kernel<<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(sn, fk_col, l, aa, *st);
   B2_CHECK_LAUNCH("b2_star_agg_kernel");
   return B2_OK;
 }

@@ -80,10 +80,22 @@ class Stats:
     repeat: float = 0.0
 
 
+NARROW_HEADROOM = 1 << 30     # device bytes an image must leave free (DeviceColumn.star_image)
+
+
+def narrow_base(stats: Stats, dtype) -> Optional[int]:
+    """Base of the 32-bit frame-of-reference image of an int64 column with these statistics: its minimum when
+    every non-NULL value lies in [vmin, vmin + 2^32), else None.  Exact: the range is taken in Python ints."""
+    if dtype != I64 or stats.vmin is None:
+        return None
+    lo, hi = int(stats.vmin), int(stats.vmax)
+    return lo if hi - lo < (1 << 32) else None
+
+
 class DeviceColumn:
     """values buffer + optional Arrow validity bitmap (stored as int32 words) on one GPU."""
 
-    __slots__ = ("data", "valid", "dtype", "logical", "n", "stats", "flags")
+    __slots__ = ("data", "valid", "dtype", "logical", "n", "stats", "flags", "base", "_image")
 
     def __init__(self, data: torch.Tensor, valid: Optional[torch.Tensor], dtype: int, logical=None, stats=None):
         self.data = data
@@ -93,6 +105,8 @@ class DeviceColumn:
         self.n = int(data.shape[0])
         self.stats = stats
         self.flags = 0
+        self.base = 0          # a B2_U32 image: the value of offset 0 (the star scans pass it beside the scan)
+        self._image = None     # (data._version, what star_image returns) once decided
 
     @property
     def device(self):
@@ -113,6 +127,31 @@ class DeviceColumn:
         if self.stats is None:
             self.stats = col_stats(self)
         return self.stats
+
+    def star_image(self) -> "DeviceColumn":
+        """What a star scan streams for this column: its 32-bit image when the column is int64 and its values
+        span less than 2^32 (narrow_base; b2_narrow_image: uint32 offsets from `base`, 0 for a NULL row, this
+        column's bitmap), else the column itself.  4 bytes per row instead of 8 in the scans, 4 more per row of
+        HBM while the image is kept.  Made on first use, on the current stream, unless the device would be left
+        with less than NARROW_HEADROOM free; kept with the column and made again, from fresh statistics, once a
+        write to the values moves the tensor's version counter.  B200SQL_NO_NARROW=1: always the column."""
+        if self.dtype != I64 or self.n == 0 or os.environ.get("B200SQL_NO_NARROW") == "1":
+            return self
+        version = self.data._version
+        if self._image is not None:
+            if self._image[0] == version:
+                return self._image[1]
+            self.stats = None              # they describe the values the old image was made of
+        base = narrow_base(self.ensure_stats(), self.dtype)
+        img = self
+        if base is not None and torch.cuda.mem_get_info(self.device)[0] >= 4 * self.n + NARROW_HEADROOM:
+            out = torch.empty(self.n, dtype=torch.int32, device=self.device)
+            st = self.as_struct()
+            L.narrow_image(C.byref(st), self.n, base, ptr(out), stream_ptr())
+            img = DeviceColumn(out, self.valid, L.U32, self.logical)
+            img.base = base
+        self._image = (version, img)
+        return img
 
     def slice(self, lo, hi):
         """Row-range view.  Only valid for lo % 32 == 0 when the column has a validity bitmap."""

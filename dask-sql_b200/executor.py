@@ -1713,8 +1713,13 @@ class PreparedStar:
             raise _NotPreparable()
         self.q, self.dev, self.cached = q, dev, cached
         self.nslots = q.grng + 1
-        # ---- launch descriptors; the ScanCtx objects keep the columns their scans point into alive
+        # ---- launch descriptors; the ScanCtx objects keep the columns their scans point into alive.  A cached
+        # plan's scans stream every int64 column -- the keys, the predicate columns, int64 aggregate inputs --
+        # as its 32-bit image where it has one (DeviceColumn.star_image); `images` remembers which, so that
+        # run() re-makes a scan whose column was written to.  A plan run once reads its columns once: making
+        # an image would cost more than it saves.
         self.keep = []
+        self.images = []          # (launch, ScanCtx, the columns its scan points into)
         self.dim_launch = []
         for part in dparts:
             if part.n == 0:
@@ -1722,7 +1727,7 @@ class PreparedStar:
             ctx = ScanCtx(part, q.dpred)
             pk_slot, g_slot = ctx.slot(q.pk_e), ctx.slot(q.ge)     # slots first: scan() snapshots the columns
             self._only_table_columns(ctx)
-            self.dim_launch.append((ctx.scan(), pk_slot, g_slot))
+            self.dim_launch.append(self._launch(ctx, pk_slot, g_slot))
             self.keep.append(ctx)
         self.fact_launch = []
         for part in fparts:
@@ -1732,7 +1737,7 @@ class PreparedStar:
             fk_slot = ctx.slot(q.fk_e)
             specs = [(ctx.slot(ka.expr), ka.op) for ka in q.plan.kaggs]
             self._only_table_columns(ctx)
-            self.fact_launch.append((ctx.scan(), fk_slot, D.make_aggs(specs), len(specs), part.n))
+            self.fact_launch.append(self._launch(ctx, fk_slot, D.make_aggs(specs), len(specs), part.n))
             self.keep.append(ctx)
         # ---- reused device buffers
         # ONE lookup buffer: every run rebuilds it in stream order, after the previous run's scan.  (Two
@@ -1848,11 +1853,30 @@ class PreparedStar:
         if self.cached and any(not k.startswith("col:") for k in ctx.index):
             raise _NotPreparable()                  # computed inputs / mask predicates are evaluated per query
 
+    def _launch(self, ctx: "ScanCtx", *args):
+        """[scan descriptor of ctx, the bases of its image columns (None: it has none), *args]: a launch of the
+        build or the probe"""
+        if not self.cached:
+            return [ctx.scan(), None, *args]
+        cols = [c.star_image() for c in ctx.cols]
+        launch = [*_image_scan(cols, ctx), *args]
+        self.images.append((launch, ctx, cols))
+        return launch
+
+    def _refresh_images(self):
+        """A column written to since the last run has a new image (or none): re-make the scans that read it."""
+        for launch, ctx, cols in self.images:
+            now = [c.star_image() for c in ctx.cols]
+            if any(a is not b for a, b in zip(now, cols)):
+                launch[0], launch[1] = _image_scan(now, ctx)
+                cols[:] = now
+
     def run(self, src) -> Part:
         q = self.q
         i = self.runs & 1
         self.runs += 1
         buf = self.lookup
+        self._refresh_images()
         main = D.cur_stream()
         sp = D.stream_ptr()
         # The host waits here until the run before the previous one has FINISHED: at most two executions
@@ -1881,10 +1905,11 @@ class PreparedStar:
             if self.dirty[ti]:
                 t.reset()
             self.dirty[ti] = True
-            for scan, fk_slot, aggs_arr, naggs, n in self.fact_launch:
+            for scan, bases, fk_slot, aggs_arr, naggs, n in self.fact_launch:
                 stats["launches"] += 1
                 ev = _kernel_event_begin("b2_star_agg_kernel", n)
-                L.star_agg(C.byref(scan), fk_slot, C.byref(self.lk), aggs_arr, naggs, C.byref(t.state), sp)
+                L.star_agg_narrow(C.byref(scan), bases, fk_slot, C.byref(self.lk), aggs_arr, naggs, C.byref(t.state),
+                                  sp)
                 _kernel_event_end(ev)
         if self.peer is not None:
             m, view = self.peer[ti]
@@ -1917,6 +1942,15 @@ class _NotPreparable(Exception):
     pass
 
 
+def _image_scan(cols, ctx: "ScanCtx"):
+    """(scan descriptor over `cols`, the int64 bases of its B2_U32 image columns for the b2_star_*_narrow entry
+    points, or None when it has none)"""
+    bases = None
+    if any(c.dtype == L.U32 for c in cols):
+        bases = (C.c_int64 * len(cols))(*[c.base for c in cols])
+    return D.make_scan(cols, ctx.terms, ctx.part.n), bases
+
+
 def _star_slot_bits(null_slot):
     """Width of the packed slots of a ranked-bitmap star lookup (include/b200sql.h, b2_star_build_mark):
     the narrowest of 16, 21 and 32 bits that holds the largest slot, null_slot.  Narrower slots keep
@@ -1937,7 +1971,7 @@ def _star_bitmap_words(prange, dn, slot_bits):
 
 
 def _star_bitmap_build(buf, launches, pmin, prange, gmin, null_slot, dn, slot_bits, sp):
-    """The ranked-bitmap lookup from (scan, pk slot, grp slot) of every dim partition, in stream order:
+    """The ranked-bitmap lookup from (scan, image bases, pk slot, grp slot) of every dim partition, in stream order:
     zero the directory (with packed slots, the slot words too: FILL ORs into them) and flags, mark every
     partition, rank, fill every partition."""
     slots_off, flags_off, _ = _star_bitmap_words(prange, dn, slot_bits)
@@ -1945,14 +1979,14 @@ def _star_bitmap_build(buf, launches, pmin, prange, gmin, null_slot, dn, slot_bi
     dirp, slots, flags = C.c_void_p(base), C.c_void_p(base + 4 * slots_off), C.c_void_p(base + 4 * flags_off)
     L.memset(dirp, 0, 4 * (flags_off if slot_bits < 32 else slots_off), sp)
     L.memset(flags, 0, 16, sp)
-    for scan, pk_slot, _ in launches:
+    for scan, bases, pk_slot, _ in launches:
         stats["launches"] += 1
-        L.star_build_mark(C.byref(scan), pk_slot, pmin, prange, dirp, flags, sp)
+        L.star_build_mark_narrow(C.byref(scan), bases, pk_slot, pmin, prange, dirp, flags, sp)
     stats["launches"] += 1
     L.star_build_rank(dirp, prange, sp)
-    for scan, pk_slot, g_slot in launches:
+    for scan, bases, pk_slot, g_slot in launches:
         stats["launches"] += 1
-        L.star_build_fill_packed(C.byref(scan), pk_slot, g_slot, pmin, prange, gmin, null_slot, dirp, slots,
+        L.star_build_fill_narrow(C.byref(scan), bases, pk_slot, g_slot, pmin, prange, gmin, null_slot, dirp, slots,
                                  slot_bits, sp)
 
 

@@ -37,8 +37,12 @@ extern "C" {
 #define B2_I64 0   /* int64  (BIGINT and narrower ints, widened at ingest) */
 #define B2_F64 1   /* float64 (DOUBLE) */
 #define B2_U8  2   /* boolean, one byte per row (0/1) */
-#define B2_U32 3   /* storage only: uint32 offsets from a base, for key-ordered join payloads
-                    * (b2_join_key_layout / b2_join_write_gather_keyed); never a column type */
+#define B2_U32 3   /* storage only: uint32 offsets from a base.  Key-ordered join payloads
+                    * (b2_join_key_layout / b2_join_write_gather_keyed, base passed beside them), and the
+                    * 32-bit image of an int64 scan column (b2_narrow_image, base passed beside the scan):
+                    * a scan loads it as the int64 (uint64)base + offset.  Only the b2_star_*_narrow entry
+                    * points take such scan columns; every other one returns B2_ERR_ARG for one.  Never a
+                    * logical column type. */
 
 #define B2_MAX_COLS   16
 #define B2_MAX_TERMS   8
@@ -80,9 +84,9 @@ extern "C" {
 #define B2_EMPTY_KEY ((int64_t)0x8000000000000000LL)
 
 typedef struct b2_col {
-  const void*    data;    /* int64_t* / double* / uint8_t* */
+  const void*    data;    /* int64_t* / double* / uint8_t* (uint32_t* for a B2_U32 scan column) */
   const uint8_t* valid;   /* Arrow validity bitmap or NULL */
-  int32_t        dtype;   /* B2_I64 / B2_F64 / B2_U8 */
+  int32_t        dtype;   /* B2_I64 / B2_F64 / B2_U8, or B2_U32 in a star scan */
   int32_t        flags;   /* B2_COL_* (0 for ordinary columns) */
 } b2_col_t;
 /* a B2_U32 key-ordered join payload in which every offset WITHOUT a build row holds 0xFFFFFFFF: the
@@ -587,6 +591,12 @@ int32_t b2_sort_by(const b2_col_t* col, int64_t n, int32_t descending, int32_t n
 int32_t b2_dense_slots(const b2_col_t* key, int64_t n, int64_t kmin, int32_t null_slot,
                        int32_t* out_slot, void* stream);
 
+/* The 32-bit frame-of-reference image of a B2_I64 column whose values all lie in [base, base + 2^32):
+ * out[i] = (uint32)((uint64)col[i] - (uint64)base), and 0 for a NULL row (the bitmap stays the column's).
+ * The star entry points *_narrow stream it as a B2_U32 scan column with `base` in their bases[] argument:
+ * 4 bytes per row instead of 8. */
+int32_t b2_narrow_image(const b2_col_t* col, int64_t n, int64_t base, uint32_t* out, void* stream);
+
 /* Build the join->group lookup of the fused pipeline from the (already filtered) build side:
  * for build row r = sel ? sel[i] : i, lookup[pk[r]-kmin] = slot_of_row[i].  Dense variant;
  * d_flags[0] = 1 on duplicate pk. */
@@ -617,6 +627,14 @@ int32_t b2_star_build_fill(const b2_scan_t* scan, int32_t pk_col, int32_t grp_co
 int32_t b2_star_build_fill_packed(const b2_scan_t* scan, int32_t pk_col, int32_t grp_col, int64_t pk_min,
                                   int64_t pk_range, int64_t grp_min, int32_t null_slot, const uint64_t* dir,
                                   uint64_t* slots, int32_t slot_bits, void* stream);
+/* b2_star_build_mark / b2_star_build_fill_packed over a scan that may hold B2_U32 images (b2_narrow_image):
+ * bases[c] (scan->ncols entries) is the base of column c where it is B2_U32, ignored elsewhere.  NULL bases:
+ * exactly the functions above, which refuse image columns. */
+int32_t b2_star_build_mark_narrow(const b2_scan_t* scan, const int64_t* bases, int32_t pk_col, int64_t pk_min,
+                                  int64_t pk_range, uint64_t* dir, int32_t* d_flags, void* stream);
+int32_t b2_star_build_fill_narrow(const b2_scan_t* scan, const int64_t* bases, int32_t pk_col, int32_t grp_col,
+                                  int64_t pk_min, int64_t pk_range, int64_t grp_min, int32_t null_slot,
+                                  const uint64_t* dir, uint64_t* slots, int32_t slot_bits, void* stream);
 /* Hash variant: table_keys = int64[cap] pre-filled with B2_EMPTY_KEY, table_slots = int32[cap].
  * d_flags[0] = 1 on duplicate pk, d_flags[1] = 1 on overflow. */
 int32_t b2_star_build_hash(const b2_col_t* pk, const int32_t* sel, int64_t n_sel,
@@ -641,6 +659,9 @@ typedef struct b2_starlookup {
  *   Aggregate(group by build cols; aggs over probe cols) <- Inner Join(fk = unique pk). */
 int32_t b2_star_agg(const b2_scan_t* scan, int32_t fk_col, const b2_starlookup_t* lk,
                     const b2_agg_t* aggs, int32_t naggs, const b2_aggstate_t* st, void* stream);
+/* b2_star_agg over a scan that may hold B2_U32 images, bases[] as for b2_star_build_mark_narrow */
+int32_t b2_star_agg_narrow(const b2_scan_t* scan, const int64_t* bases, int32_t fk_col, const b2_starlookup_t* lk,
+                           const b2_agg_t* aggs, int32_t naggs, const b2_aggstate_t* st, void* stream);
 
 #ifdef __cplusplus
 }

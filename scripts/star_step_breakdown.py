@@ -3,9 +3,13 @@
 in 8 partitions, 10M dim rows, 1M groups) timed with CUDA events per phase of PreparedStar.run (build /
 scan / ...) and per launch of the ranked-bitmap build (the memsets, every mark, the rank, every fill),
 next to the step time and the b2_star_agg_kernel time.  One JSON line per phase and per launch, in ms
-per step, each carrying the card's name and power limit.
+per step and per call, each carrying the card's name and power limit; then one "bytes" line: the bytes per
+fact and per dim row that the prepared plan's scans physically read (int64 columns streamed as their 32-bit
+images, DeviceColumn.star_image, unless B200SQL_NO_NARROW=1) against the logical 24 B per fact row that
+bench.py's roofline divides by, and the probe's physical bandwidth from the b2_star_agg_kernel time.
 
     python scripts/star_step_breakdown.py --steps 10 --warmup 3
+    B200SQL_NO_NARROW=1 python scripts/star_step_breakdown.py --steps 10 --warmup 3
 
 B200SQL_LIB selects another build of libb200sql.so (the C-ABI is the same), so two builds can be
 compared by the same Python."""
@@ -42,7 +46,8 @@ def main():
     ap.add_argument("--rows", type=float, default=1e9)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--label", default=os.environ.get("B200SQL_LIB", "in-tree"))
+    ap.add_argument("--label", default=os.environ.get("B200SQL_LIB", "in-tree") +
+                    (" int64" if os.environ.get("B200SQL_NO_NARROW") == "1" else " images"))
     args = ap.parse_args()
     if args.steps < 1:
         ap.error("--steps must be >= 1")
@@ -85,8 +90,8 @@ def main():
             return rc
         return call
 
-    for attr, name in (("memset", "memset"), ("star_build_mark", "mark"), ("star_build_rank", "rank"),
-                       ("star_build_fill_packed", "fill")):
+    for attr, name in (("memset", "memset"), ("star_build_mark_narrow", "mark"), ("star_build_rank", "rank"),
+                       ("star_build_fill_narrow", "fill")):
         setattr(L, attr, timed(name, getattr(L, attr)))
     build = executor._star_bitmap_build
 
@@ -124,7 +129,8 @@ def main():
 
     def emit(kind, name, ms, count):
         print(json.dumps({"kind": kind, "name": name, "ms_per_step": round(ms / args.steps, 4),
-                          "calls_per_step": count / args.steps, **common}), flush=True)
+                          "calls_per_step": count / args.steps, "ms_per_call": round(ms / count, 4), **common}),
+              flush=True)
 
     emit("step", "step", e0.elapsed_time(e1), args.steps)
     for kind, recs in (("phase", [(r[0], r[1], r[2]) for r in pev]), ("launch", launches),
@@ -135,6 +141,23 @@ def main():
             cnt[name] = cnt.get(name, 0) + 1
         for name in tot:
             emit(kind, name, tot[name], cnt[name])
+
+    # bytes per row as the plan's scan descriptors point at them (validity bitmaps: 1/8 B per row)
+    width = {L.I64: 8, L.F64: 8, L.U8: 1, L.U32: 4}
+    prep = executor.PreparedStar._live[-1]
+
+    def row_bytes(launches):
+        s = launches[0][0]
+        return sum(width[s.cols[i].dtype] + (0.125 if s.cols[i].valid else 0) for i in range(s.ncols))
+
+    images = [(s.cols[i].dtype == L.U32) for s, *_ in prep.fact_launch + prep.dim_launch for i in range(s.ncols)]
+    fact_b = row_bytes(prep.fact_launch)
+    probe_ms = sum(r[2].elapsed_time(r[3]) for r in kev if r[0] == "b2_star_agg_kernel") / args.steps
+    print(json.dumps({"kind": "bytes", "fact_bytes_per_row": fact_b, "fact_bytes_per_row_logical": 24,
+                      "dim_bytes_per_row": row_bytes(prep.dim_launch), "image_columns": sum(images),
+                      "scan_columns": len(images), "probe_gbs_physical": round(n * fact_b / probe_ms / 1e6, 1),
+                      "probe_frac_of_3350_gbs": round(n * fact_b / probe_ms / 1e6 / 3350, 3),
+                      "hbm_allocated_gb": round(torch.cuda.memory_allocated(dev) / 1e9, 2), **common}), flush=True)
 
 
 if __name__ == "__main__":
