@@ -131,8 +131,6 @@ _lib.b2_num_tiles.restype = C.c_int64
 _lib.b2_num_tiles.argtypes = [C.c_int64]
 _lib.b2_stats_ws_bytes.restype = C.c_int64
 _lib.b2_scan_agg_ws_bytes.restype = C.c_int64
-_lib.b2_join_onepass_ws_bytes.restype = C.c_int64
-_lib.b2_join_onepass_ws_bytes.argtypes = [C.c_int64]
 _lib.b2_range_partition_ws_bytes.restype = C.c_int64
 _lib.b2_range_partition_ws_bytes.argtypes = [C.c_int32]
 _lib.b2_f64_to_ordered.restype = C.c_int64
@@ -182,7 +180,7 @@ _SIGS = {
                                    _P, _P, C.c_int32, C.POINTER(C.c_int32), C.POINTER(_P), C.POINTER(_P),
                                    C.c_int32, C.POINTER(Col), C.POINTER(C.c_int64), C.POINTER(_P), C.POINTER(_P),
                                    _P],
-    "b2_join_onepass": [C.POINTER(Scan), C.POINTER(C.c_int32), C.POINTER(JoinTable), C.c_int32, C.c_int32, _P, C.c_int32,
+    "b2_join_onepass": [C.POINTER(Scan), C.POINTER(C.c_int32), C.POINTER(JoinTable), C.c_int32, _P, C.c_int32,
                         C.POINTER(C.c_int32), C.POINTER(_P), C.POINTER(_P), C.c_int32, C.POINTER(Col),
                         C.POINTER(C.c_int64), C.POINTER(_P), C.POINTER(_P), _P],
     "b2_join_agg": [C.POINTER(Scan), C.c_int32, C.POINTER(JoinTable), C.c_int32, C.POINTER(Col), C.POINTER(C.c_int64),
@@ -219,7 +217,7 @@ _SIGS = {
 }
 
 EXPORTS = sorted(list(_SIGS) + ["b2_last_error", "b2_num_tiles", "b2_stats_ws_bytes", "b2_scan_agg_ws_bytes",
-                                "b2_sort_ws_bytes", "b2_join_onepass_ws_bytes", "b2_range_partition_ws_bytes",
+                                "b2_sort_ws_bytes", "b2_range_partition_ws_bytes",
                                 "b2_f64_to_ordered", "b2_ordered_to_f64"])
 
 
@@ -284,7 +282,6 @@ join_write_gather = _wrap("b2_join_write_gather")
 join_write_gather_keyed = _wrap("b2_join_write_gather_keyed")
 join_key_layout = _wrap("b2_join_key_layout")
 join_onepass = _wrap("b2_join_onepass")
-join_onepass_ws_bytes = _lib.b2_join_onepass_ws_bytes
 join_agg = _wrap("b2_join_agg")
 range_partition = _wrap("b2_range_partition")
 range_partition_hist = _wrap("b2_range_partition_hist")

@@ -73,49 +73,6 @@ __device__ __forceinline__ uint64_t b2_mix64(uint64_t k) {  // murmur3 fmix64
   return k;
 }
 
-// ---- decoupled look-back (single-pass order-preserving compaction) -------------------------------
-// status[tile]: bits 63..62 = 0 not ready / 1 tile aggregate / 2 inclusive prefix, low 62 bits = value.
-// Called by the 32 lanes of one warp once the tile's own count `agg` is known; publishes it, sums the
-// predecessors' aggregates back to the nearest inclusive prefix and returns the tile's exclusive
-// prefix.  Only the 64-bit status word is exchanged, so relaxed volatile accesses suffice.  Progress:
-// the grid is resident (b2_wave_grid) and every block takes its tiles in increasing order, so the
-// lowest unfinished tile never waits.
-#define B2_LB_AGG (1ULL << 62)
-#define B2_LB_PREFIX (2ULL << 62)
-#define B2_LB_MASK ((1ULL << 62) - 1)
-__device__ __forceinline__ uint64_t b2_ld_volatile_u64(const uint64_t* p) {
-  uint64_t v;
-  asm volatile("ld.volatile.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void b2_st_volatile_u64(uint64_t* p, uint64_t v) {
-  asm volatile("st.volatile.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-__device__ __forceinline__ int64_t b2_lookback(uint64_t* __restrict__ status, int64_t tile, int64_t agg, int lane) {
-  if (tile == 0) {
-    if (lane == 0) b2_st_volatile_u64(status, B2_LB_PREFIX | (uint64_t)agg);
-    return 0;
-  }
-  if (lane == 0) b2_st_volatile_u64(status + tile, B2_LB_AGG | (uint64_t)agg);
-  int64_t excl = 0;
-  for (int64_t t = tile - 1;; t -= 32) {
-    const int64_t idx = t - lane;                       // lane 0 = nearest predecessor
-    uint64_t v = B2_LB_PREFIX;                          // before tile 0: prefix 0
-    if (idx >= 0) {
-      do { v = b2_ld_volatile_u64(status + idx); } while ((v >> 62) == 0);
-    }
-    const uint32_t pmask = __ballot_sync(FULL_MASK, (v >> 62) == 2);
-    const int first = pmask ? __ffs(pmask) - 1 : 31;    // nearest lane holding an inclusive prefix
-    int64_t val = lane <= first ? (int64_t)(v & B2_LB_MASK) : 0;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) val += __shfl_xor_sync(FULL_MASK, val, o);
-    excl += val;
-    if (pmask) break;
-  }
-  if (lane == 0) b2_st_volatile_u64(status + tile, B2_LB_PREFIX | (uint64_t)(excl + agg));
-  return excl;
-}
-
 __device__ __forceinline__ bool b2_bit(const uint8_t* __restrict__ bm, int64_t i) {
   return (bm[i >> 3] >> (i & 7)) & 1;
 }

@@ -426,10 +426,11 @@ b2_join_write_kernel(const __grid_constant__ b2_scan_t s, const __grid_constant_
 }
 
 // ---- single-pass probe of a direct-address table ------------------------------------------------
-// Every probe row emits at most one output row, so one kernel can do the whole join: each 2048-row
-// tile counts its emitting rows, learns its output offset by a decoupled look-back over the tiles
-// before it (b2_lookback) and writes.  The loads are front-loaded so that a tile costs two
-// dependent memory round trips instead of one per gathered column:
+// Every probe row emits at most one output row, so one kernel can do the whole join: each warp owns
+// 256 consecutive probe rows of a 2048-row tile, ranks its emitting rows by ballot and reserves its
+// output range with one atomicAdd on *total.  Rows of one warp batch stay contiguous and in probe
+// order; the batches land in the order the warps reserve.  The loads are front-loaded so that a
+// batch costs two dependent memory round trips instead of one per gathered column:
 //   trip 1: probe key, predicate columns and the first other 8-byte probe column (streaming)
 //   trip 2: presence word and -- on a key-ordered table (dense == 2) -- the first build column's
 //           payload at the key offset, fetched speculatively together with the presence word
@@ -437,21 +438,11 @@ b2_join_write_kernel(const __grid_constant__ b2_scan_t s, const __grid_constant_
 #define B2_JOP_R 8
 #define B2_JOP_TILE (B2_BLOCK * B2_JOP_R)
 
-#ifndef B2_JOP_MINB
-#define B2_JOP_MINB 2
-#endif
-__global__ void __launch_bounds__(B2_BLOCK, B2_JOP_MINB)
+__global__ void __launch_bounds__(B2_BLOCK, 2)
 b2_join_onepass_kernel(const __grid_constant__ b2_scan_t s, int key_col, const __grid_constant__ b2_jointable_t jt,
-                       int mode, int64_t ntiles, uint64_t* __restrict__ status, const int64_t* __restrict__ tile_off,
-                       const uint32_t* __restrict__ match_mask, int64_t* __restrict__ total,
+                       int mode, int64_t ntiles, unsigned long long* __restrict__ total,
                        const __grid_constant__ b2_joingather_arg g) {
-  // tile_off != NULL: offsets were counted by b2_join_count8_kernel + scan (three launches, still no
-  // host round trip); tile_off == NULL && status != NULL: decoupled look-back over `status` (one launch);
-  // both NULL: every warp reserves its output range with one atomicAdd on *total (one launch, every
-  // input byte read once, output order = order in which the warps got there)
   constexpr int R = B2_JOP_R;
-  __shared__ int64_t sh[B2_WARPS];
-  __shared__ int64_t sh_excl;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const uint32_t lt_mask = (1u << lane) - 1;
   const b2_col_t& kc = s.cols[key_col];
@@ -466,19 +457,7 @@ b2_join_onepass_kernel(const __grid_constant__ b2_scan_t s, int key_col, const _
   for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const int64_t row0 = tile * B2_JOP_TILE + (int64_t)warp * (32 * R) + lane;
     bool full;
-    uint32_t bits, known = 0;
-    if (match_mask) {
-      // counted mode: which rows found a build row is already known; an INNER / SEMI probe then
-      // touches only the rows it emits (no predicate columns, no loads for the others)
-      const uint32_t* mw = match_mask + ((row0 - lane) >> 5);
-#pragma unroll
-      for (int j = 0; j < R; ++j)
-        if (row0 - lane + (int64_t)j * 32 < s.n) known |= ((__ldg(mw + j) >> lane) & 1u) << j;
-      if (mode == B2_JOIN_INNER || mode == B2_JOIN_SEMI) { bits = known; full = false; }
-      else bits = b2_eval_terms<R>(s, row0, full);
-    } else {
-      bits = b2_eval_terms<R>(s, row0, full);
-    }
+    const uint32_t bits = b2_eval_terms<R>(s, row0, full);
     int64_t key[R], pre[R];
     b2_load_batch<R>(kc, row0, bits, full, key);
     if (preA >= 0) b2_load_batch64<R>(s.cols[g.probe_cols[preA]].data, row0, bits, full, pre);
@@ -487,19 +466,7 @@ b2_join_onepass_kernel(const __grid_constant__ b2_scan_t s, int key_col, const _
 
     int32_t brow[R];
     int64_t pay[R];
-    if (match_mask) {
-#pragma unroll
-      for (int j = 0; j < R; ++j) {
-        const uint64_t d = (uint64_t)key[j] - (uint64_t)jt.kmin;
-        const bool ok = (known >> j) & 1;
-        brow[j] = !ok ? -1 : (jt.dense == 2 ? (int32_t)d : b2_ld_keep_i32(jt.lookup + d));
-        pay[j] = 0;
-        if (spec && ok) {
-          pay[j] = spec32 ? (int64_t)(uint32_t)b2_ld_keep_i32(reinterpret_cast<const int32_t*>(g.build_cols[0].data) + d)
-                          : b2_ld_keep_i64(reinterpret_cast<const int64_t*>(g.build_cols[0].data) + d);
-        }
-      }
-    } else if (jt.dense == 2) {
+    if (jt.dense == 2) {
       uint32_t word[R];
 #pragma unroll
       for (int j = 0; j < R; ++j) {
@@ -535,7 +502,7 @@ b2_join_onepass_kernel(const __grid_constant__ b2_scan_t s, int key_col, const _
       default: emit = bits & ~matched; break;  // ANTI
     }
 
-    // ---- positions: ballot ranks inside the warp, warps inside the tile, tiles by look-back
+    // ---- positions: ballot ranks inside the warp, one reservation per warp batch
     int32_t rel[R];
     int wtotal = 0;
 #pragma unroll
@@ -544,33 +511,9 @@ b2_join_onepass_kernel(const __grid_constant__ b2_scan_t s, int key_col, const _
       rel[j] = ((emit >> j) & 1) ? wtotal + __popc(b & lt_mask) : -1;
       wtotal += __popc(b);
     }
-    int64_t off;
-    if (tile_off) {
-      // counted mode: warp-granular offsets, no barrier -- warps of a block drift freely
-      off = __ldg(tile_off + tile * B2_WARPS + warp);
-      if (tile == ntiles - 1 && threadIdx.x == 0) *total = tile_off[ntiles * B2_WARPS];
-    } else if (!status) {
-      unsigned long long r = 0;
-      if (lane == 0 && wtotal) r = atomicAdd(reinterpret_cast<unsigned long long*>(total), (unsigned long long)wtotal);
-      off = (int64_t)__shfl_sync(FULL_MASK, r, 0);
-    } else {
-      if (lane == 0) sh[warp] = wtotal;
-      __syncthreads();
-      if (warp == 0) {
-        int64_t agg = 0;
-#pragma unroll
-        for (int w = 0; w < B2_WARPS; ++w) agg += sh[w];
-        const int64_t ex = b2_lookback(status, tile, agg, lane);
-        if (lane == 0) {
-          sh_excl = ex;
-          if (tile == ntiles - 1) *total = ex + agg;
-        }
-      }
-      __syncthreads();
-      off = sh_excl;
-      for (int w = 0; w < warp; ++w) off += sh[w];
-      __syncthreads();
-    }
+    unsigned long long r = 0;
+    if (lane == 0 && wtotal) r = atomicAdd(total, (unsigned long long)wtotal);
+    const int64_t off = (int64_t)__shfl_sync(FULL_MASK, r, 0);
 
     // ---- probe-side columns
     for (int k = 0; k < g.nprobe; ++k) {
@@ -657,21 +600,21 @@ b2_join_onepass_kernel(const __grid_constant__ b2_scan_t s, int key_col, const _
 // ---- streaming probe, specialised --------------------------------------------------------------------
 // The shape of C3 (and of most star-schema joins): INNER / SEMI probe of a key-ordered table, output =
 // [probe key] [one more 8-byte probe column] [one build column], nothing nullable.  One launch, every
-// input byte read once, no match mask, no count pass, no block barrier:
+// input byte read once, no count pass:
 //   trip 1  key + predicate columns + the probe column      (streaming, coalesced)
 //   trip 2  presence word + payload at the key offset        (L2-resident table, evict_last)
-//   ranks   ballots inside the warp; ONE atomicAdd per warp batch reserves the output range
+//   ranks   ballots inside the warp, warp counts summed in shared memory; ONE atomicAdd per 2048-row
+//           tile reserves the output range
 //   stores  streaming (evict_first), consecutive lanes -> consecutive rows of the reserved range
-// Output rows of one warp batch stay in probe order; batches land in the order the warps reserve.
-// SQL leaves the row order of a join unspecified (the reference's tests sort before comparing,
-// tests/integration/test_compatibility.py:7-9); callers that want probe order use the counted mode.
+// Output rows of one tile stay in probe order; tiles land in the order their CTAs reserve.  SQL leaves
+// the row order of a join unspecified (the reference's tests sort before comparing,
+// tests/integration/test_compatibility.py:7-9).
 // BMODE: how the build column is stored -- 0 none, 1 eight bytes, 2 uint32 offsets (+ presence bitmap),
 // 3 uint32 offsets in which 0xFFFFFFFF marks "no build row" (B2_COL_SENTINEL: no bitmap access at all)
-// CTA_RES: the 8 warps of a tile reserve their output range together (two barriers per 2048-row tile, one
-// atomic) instead of one atomic per warp batch: *total is ONE address, and the L2 serves same-address
-// atomics one at a time (~1.5 ns each, scripts/microbench/redg.cu) -- 488k reservations per 125M-row
-// partition were most of the kernel's time.
-template <bool HAS_P, int BMODE, bool OUT_KEY, bool CTA_RES>
+// The 8 warps of a tile reserve together (two barriers, one atomic) rather than one atomic per warp
+// batch: *total is ONE address, and the L2 serves same-address atomics one at a time (~1.5 ns each,
+// scripts/microbench/redg.cu) -- 488k reservations per 125M-row partition were most of the kernel's time.
+template <bool HAS_P, int BMODE, bool OUT_KEY>
 __global__ void __launch_bounds__(B2_BLOCK, 3)
 b2_join_stream_kernel(const __grid_constant__ b2_scan_t s, int key_col, int p_col, const __grid_constant__ b2_jointable_t jt,
                       const void* __restrict__ payload, int64_t pay_base, int64_t ntiles, int64_t* __restrict__ out_key,
@@ -728,26 +671,19 @@ b2_join_stream_kernel(const __grid_constant__ b2_scan_t s, int key_col, int p_co
       rel[j] = ((emit >> j) & 1) ? wtotal + __popc(b & lt_mask) : -1;
       wtotal += __popc(b);
     }
-    int64_t off;
-    if (CTA_RES) {
-      // double-buffered by tile parity: a warp that runs ahead writes the OTHER buffer
-      if (lane == 0) sh_cnt[phase][warp] = wtotal;
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        int t = 0;
+    // double-buffered by tile parity: a warp that runs ahead writes the OTHER buffer
+    if (lane == 0) sh_cnt[phase][warp] = wtotal;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      int t = 0;
 #pragma unroll
-        for (int w = 0; w < B2_WARPS; ++w) t += sh_cnt[phase][w];
-        sh_base[phase] = t ? (long long)atomicAdd(total, (unsigned long long)t) : 0;
-      }
-      __syncthreads();
-      off = sh_base[phase];
-      for (int w = 0; w < warp; ++w) off += sh_cnt[phase][w];
-      phase ^= 1;
-    } else {
-      unsigned long long r = 0;
-      if (lane == 0 && wtotal) r = atomicAdd(total, (unsigned long long)wtotal);
-      off = (int64_t)__shfl_sync(FULL_MASK, r, 0);
+      for (int w = 0; w < B2_WARPS; ++w) t += sh_cnt[phase][w];
+      sh_base[phase] = t ? (long long)atomicAdd(total, (unsigned long long)t) : 0;
     }
+    __syncthreads();
+    int64_t off = sh_base[phase];
+    for (int w = 0; w < warp; ++w) off += sh_cnt[phase][w];
+    phase ^= 1;
 #pragma unroll
     for (int j = 0; j < R; ++j) {
       if (rel[j] < 0) continue;
@@ -755,33 +691,6 @@ b2_join_stream_kernel(const __grid_constant__ b2_scan_t s, int key_col, int p_co
       if (HAS_P) b2_st_stream(out_p + off + rel[j], pv[j]);
       if (HAS_B) b2_st_stream(out_b + off + rel[j], BMODE >= 2 ? pay_base + pay[j] : pay[j]);
     }
-  }
-}
-
-// per-WARP emit counts for b2_join_onepass_kernel's geometry (a warp owns 256 consecutive probe rows of
-// its 2048-row tile) plus the match mask; reads key + presence only.  With warp-granular offsets the
-// write pass needs no block barrier at all.
-__global__ void __launch_bounds__(B2_BLOCK, 4)
-b2_join_count8_kernel(const __grid_constant__ b2_scan_t s, int key_col, const __grid_constant__ b2_jointable_t jt,
-                      int mode, int64_t ntiles, int64_t* __restrict__ warp_cnt, uint32_t* __restrict__ match_mask) {
-  // match_mask: one bit per probe row (word w covers rows 32w..32w+31) = "found its build row"; the
-  // write pass reads it instead of probing the table a second time
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    const int64_t row0 = tile * B2_JOP_TILE + (int64_t)warp * (32 * B2_JOP_R) + lane;
-    int32_t brow[B2_JOP_R];
-    int c = __popc(b2_dense_probe<B2_JOP_R>(s, key_col, jt, mode, row0, brow));
-    uint32_t mine = 0;   // lane j keeps the ballot of batch row j
-#pragma unroll
-    for (int j = 0; j < B2_JOP_R; ++j) {
-      const uint32_t b = __ballot_sync(FULL_MASK, brow[j] >= 0);
-      if (lane == j) mine = b;
-    }
-    const int64_t w0 = (row0 - lane) >> 5;
-    if (lane < B2_JOP_R && (w0 + lane) * 32 < s.n) match_mask[w0 + lane] = mine;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(FULL_MASK, c, o);
-    if (lane == 0) warp_cnt[tile * B2_WARPS + warp] = c;
   }
 }
 
@@ -950,21 +859,15 @@ int32_t b2_join_write_gather_keyed(const b2_scan_t* scan, const int32_t* probe_k
   return B2_OK;
 }
 
-static inline int64_t b2_jop_tiles(int64_t n) { return n > 0 ? (n + B2_JOP_TILE - 1) / B2_JOP_TILE : 0; }
-int64_t b2_join_onepass_ws_bytes(int64_t n) {
-  // [total][8*ntiles+1 warp offsets (or ntiles look-back status words)][match mask: 1 bit per probe row]
-  return 8 * (2 + B2_WARPS * b2_jop_tiles(n)) + 8 * ((n > 0 ? n : 0) / 64 + 1);
-}
-
 int32_t b2_join_onepass(const b2_scan_t* scan, const int32_t* probe_keys, const b2_jointable_t* jt, int32_t mode,
-                        int32_t lookback, void* d_ws, int32_t nprobe, const int32_t* probe_cols,
+                        int64_t* d_total, int32_t nprobe, const int32_t* probe_cols,
                         void* const* probe_out, uint32_t* const* probe_valid, int32_t nbuild,
                         const b2_col_t* build_cols, const int64_t* build_base, void* const* build_out,
                         uint32_t* const* build_valid, void* stream) {
   b2_probekeys_arg pk;
   int32_t rc = b2_check_join(scan, probe_keys, jt, mode, &pk);
   if (rc) return rc;
-  B2_REQUIRE(d_ws, "null argument");
+  B2_REQUIRE(d_total, "null argument");
   B2_REQUIRE(jt->dense, "single-pass probe needs a direct-address table");
   b2_joingather_arg g;
   rc = b2_fill_joingather(scan, jt, mode, nprobe, probe_cols, probe_out, probe_valid, nbuild, build_cols, build_base,
@@ -973,83 +876,58 @@ int32_t b2_join_onepass(const b2_scan_t* scan, const int32_t* probe_keys, const 
   const int64_t ntiles = (scan->n + B2_JOP_TILE - 1) / B2_JOP_TILE;
   if (ntiles <= 0) return B2_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  int64_t* total = reinterpret_cast<int64_t*>(d_ws);      // ws[0]; ws[1 .. ntiles+1] = status words / tile offsets
-  int64_t* tiles = total + 1;
-  int grid = b2_wave_grid(b2_join_onepass_kernel, B2_BLOCK, ntiles);
-  if (lookback == 2) {
-    // unordered single pass.  Specialised kernel when the shape is [key] [<=1 more probe column] [<=1 build
-    // column] on a key-ordered table with nothing nullable; the generic kernel otherwise.
-    const b2_col_t& kc = scan->cols[pk.cols[0]];
-    bool fits = jt->dense == 2 && (mode == B2_JOIN_INNER || mode == B2_JOIN_SEMI) && kc.dtype == B2_I64 && !kc.valid &&
-                nbuild <= 1 && nprobe <= 2;
-    int p_col = -1, key_out = -1, p_out = -1;
-    for (int k = 0; fits && k < nprobe; ++k) {
-      const b2_col_t& c = scan->cols[g.probe_cols[k]];
-      if (g.probe_valid[k] || c.valid || c.dtype == B2_U8) fits = false;
-      else if (g.probe_cols[k] == pk.cols[0] && key_out < 0) key_out = k;
-      else if (p_col < 0) { p_col = g.probe_cols[k]; p_out = k; }
-      else fits = false;
-    }
-    if (fits && nbuild == 1)
-      fits = !g.build_valid[0] && !g.build_cols[0].valid && g.build_cols[0].dtype != B2_U8;
-    if (fits) {
-      const bool hp = p_col >= 0, hb = nbuild == 1, ok = key_out >= 0;
-      int bmode = 0;
-      if (hb) bmode = g.build_cols[0].dtype != B2_U32 ? 1 : ((g.build_cols[0].flags & B2_COL_SENTINEL) ? 3 : 2);
-      const void* payload = hb ? g.build_cols[0].data : nullptr;
-      const int64_t base = hb ? g.build_base[0] : 0;
-      int64_t* o_key = ok ? reinterpret_cast<int64_t*>(g.probe_out[key_out]) : nullptr;
-      int64_t* o_p = hp ? reinterpret_cast<int64_t*>(g.probe_out[p_out]) : nullptr;
-      int64_t* o_b = hb ? reinterpret_cast<int64_t*>(g.build_out[0]) : nullptr;
-      unsigned long long* tot = reinterpret_cast<unsigned long long*>(total);
-      bool cta_res = true;   // B200SQL_JOIN_RESERVE=warp: one atomic per warp batch (A/B)
-      if (const char* e = getenv("B200SQL_JOIN_RESERVE")) cta_res = strcmp(e, "warp") != 0;
+  unsigned long long* total = reinterpret_cast<unsigned long long*>(d_total);
+  // specialised kernel when the shape is [key] [<=1 more probe column] [<=1 build column] on a
+  // key-ordered table with nothing nullable; the generic kernel otherwise
+  const b2_col_t& kc = scan->cols[pk.cols[0]];
+  bool fits = jt->dense == 2 && (mode == B2_JOIN_INNER || mode == B2_JOIN_SEMI) && kc.dtype == B2_I64 && !kc.valid &&
+              nbuild <= 1 && nprobe <= 2;
+  int p_col = -1, key_out = -1, p_out = -1;
+  for (int k = 0; fits && k < nprobe; ++k) {
+    const b2_col_t& c = scan->cols[g.probe_cols[k]];
+    if (g.probe_valid[k] || c.valid || c.dtype == B2_U8) fits = false;
+    else if (g.probe_cols[k] == pk.cols[0] && key_out < 0) key_out = k;
+    else if (p_col < 0) { p_col = g.probe_cols[k]; p_out = k; }
+    else fits = false;
+  }
+  if (fits && nbuild == 1)
+    fits = !g.build_valid[0] && !g.build_cols[0].valid && g.build_cols[0].dtype != B2_U8;
+  if (fits) {
+    const bool hp = p_col >= 0, hb = nbuild == 1, ok = key_out >= 0;
+    int bmode = 0;
+    if (hb) bmode = g.build_cols[0].dtype != B2_U32 ? 1 : ((g.build_cols[0].flags & B2_COL_SENTINEL) ? 3 : 2);
+    const void* payload = hb ? g.build_cols[0].data : nullptr;
+    const int64_t base = hb ? g.build_base[0] : 0;
+    int64_t* o_key = ok ? reinterpret_cast<int64_t*>(g.probe_out[key_out]) : nullptr;
+    int64_t* o_p = hp ? reinterpret_cast<int64_t*>(g.probe_out[p_out]) : nullptr;
+    int64_t* o_b = hb ? reinterpret_cast<int64_t*>(g.build_out[0]) : nullptr;
 #define B2_JS_LAUNCH(HP, BM, OK)                                                                                 \
-      do {                                                                                                        \
-        if (cta_res) {                                                                                            \
-          int sg = b2_wave_grid(b2_join_stream_kernel<HP, BM, OK, true>, B2_BLOCK, ntiles);                       \
-          b2_join_stream_kernel<HP, BM, OK, true><<<sg, B2_BLOCK, 0, st>>>(*scan, pk.cols[0], hp ? p_col : 0, *jt, \
-                                                                     payload, base, ntiles, o_key, o_p, o_b, tot); \
-        } else {                                                                                                  \
-          int sg = b2_wave_grid(b2_join_stream_kernel<HP, BM, OK, false>, B2_BLOCK, ntiles);                      \
-          b2_join_stream_kernel<HP, BM, OK, false><<<sg, B2_BLOCK, 0, st>>>(*scan, pk.cols[0], hp ? p_col : 0, *jt, \
-                                                                     payload, base, ntiles, o_key, o_p, o_b, tot); \
-        }                                                                                                         \
-      } while (0)
-#define B2_JS_BM(HP, OK)                                                                                          \
-      do {                                                                                                        \
-        if (bmode == 0) B2_JS_LAUNCH(HP, 0, OK);                                                                  \
-        else if (bmode == 1) B2_JS_LAUNCH(HP, 1, OK);                                                             \
-        else if (bmode == 2) B2_JS_LAUNCH(HP, 2, OK);                                                             \
-        else B2_JS_LAUNCH(HP, 3, OK);                                                                             \
-      } while (0)
-      if (!hp && !hb && !ok) fits = false;
-      else if (hp && ok) B2_JS_BM(true, true);
-      else if (hp) B2_JS_BM(true, false);
-      else if (ok) B2_JS_BM(false, true);
-      else B2_JS_BM(false, false);
+    do {                                                                                                         \
+      int sg = b2_wave_grid(b2_join_stream_kernel<HP, BM, OK>, B2_BLOCK, ntiles);                                \
+      b2_join_stream_kernel<HP, BM, OK><<<sg, B2_BLOCK, 0, st>>>(*scan, pk.cols[0], hp ? p_col : 0, *jt,         \
+                                                                 payload, base, ntiles, o_key, o_p, o_b, total); \
+    } while (0)
+#define B2_JS_BM(HP, OK)                                                                                         \
+    do {                                                                                                         \
+      if (bmode == 0) B2_JS_LAUNCH(HP, 0, OK);                                                                   \
+      else if (bmode == 1) B2_JS_LAUNCH(HP, 1, OK);                                                              \
+      else if (bmode == 2) B2_JS_LAUNCH(HP, 2, OK);                                                              \
+      else B2_JS_LAUNCH(HP, 3, OK);                                                                              \
+    } while (0)
+    if (!hp && !hb && !ok) fits = false;
+    else if (hp && ok) B2_JS_BM(true, true);
+    else if (hp) B2_JS_BM(true, false);
+    else if (ok) B2_JS_BM(false, true);
+    else B2_JS_BM(false, false);
 #undef B2_JS_BM
 #undef B2_JS_LAUNCH
-      if (fits) {
-        B2_CHECK_LAUNCH("b2_join_stream_kernel");
-        return B2_OK;
-      }
+    if (fits) {
+      B2_CHECK_LAUNCH("b2_join_stream_kernel");
+      return B2_OK;
     }
-    b2_join_onepass_kernel<<<grid, B2_BLOCK, 0, st>>>(*scan, pk.cols[0], *jt, mode, ntiles, nullptr, nullptr, nullptr,
-                                                      total, g);
-  } else if (lookback) {
-    b2_join_onepass_kernel<<<grid, B2_BLOCK, 0, st>>>(*scan, pk.cols[0], *jt, mode, ntiles,
-                                                      reinterpret_cast<uint64_t*>(tiles), nullptr, nullptr, total, g);
-  } else {
-    int cgrid = b2_wave_grid(b2_join_count8_kernel, B2_BLOCK, ntiles);
-    uint32_t* mask = reinterpret_cast<uint32_t*>(tiles + ntiles * B2_WARPS + 1);
-    b2_join_count8_kernel<<<cgrid, B2_BLOCK, 0, st>>>(*scan, pk.cols[0], *jt, mode, ntiles, tiles, mask);
-    B2_CHECK_LAUNCH("b2_join_count8_kernel");
-    b2_exclusive_scan_kernel<<<1, B2_SCAN_THREADS, 0, st>>>(tiles, ntiles * B2_WARPS);
-    B2_CHECK_LAUNCH("b2_exclusive_scan_kernel");
-    b2_join_onepass_kernel<<<grid, B2_BLOCK, 0, st>>>(*scan, pk.cols[0], *jt, mode, ntiles, nullptr, tiles, mask,
-                                                      total, g);
   }
+  int grid = b2_wave_grid(b2_join_onepass_kernel, B2_BLOCK, ntiles);
+  b2_join_onepass_kernel<<<grid, B2_BLOCK, 0, st>>>(*scan, pk.cols[0], *jt, mode, ntiles, total, g);
   B2_CHECK_LAUNCH("b2_join_onepass_kernel");
   return B2_OK;
 }

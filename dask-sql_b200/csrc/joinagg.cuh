@@ -168,8 +168,8 @@ __device__ __forceinline__ void b2_join_agg_body(const b2_scan_t& s, const b2_gl
   }
 }
 
-template <int MINB>   // CTAs per SM the register allocation aims for: 2 = no spills (116 regs), 3 = 80 regs + ~270 B spills
-__global__ void __launch_bounds__(B2_BLOCK, MINB)
+// three CTAs per SM: 80 registers and a few hundred bytes of spills, by design (DESIGN §4)
+__global__ void __launch_bounds__(B2_BLOCK, 3)
 b2_join_agg_kernel(const __grid_constant__ b2_scan_t s, int key_col, const __grid_constant__ b2_jointable_t jt,
                    const __grid_constant__ b2_joinagg_arg ja, b2_partial* __restrict__ partials) {
   __shared__ int64_t sh_acc[B2_MAX_AGGS][B2_BLOCK];
@@ -390,18 +390,9 @@ int32_t b2_join_agg(const b2_scan_t* scan, int32_t probe_key, const b2_jointable
     }
   }
   int64_t nblk = (scan->n + B2_JA_ROWS_PER_BLOCK - 1) / B2_JA_ROWS_PER_BLOCK;
-  int minb = 3;
-  if (const char* e = getenv("B200SQL_JA_MINB")) minb = atoi(e) == 2 ? 2 : 3;
-  int grid;
-  if (minb == 2) {
-    grid = b2_wave_grid(b2_join_agg_kernel<2>, B2_BLOCK, nblk);
-    if (grid > B2_MAX_PARTIALS) grid = B2_MAX_PARTIALS;
-    b2_join_agg_kernel<2><<<grid, B2_BLOCK, 0, st>>>(*scan, probe_key, *jt, ja, partials);
-  } else {
-    grid = b2_wave_grid(b2_join_agg_kernel<3>, B2_BLOCK, nblk);
-    if (grid > B2_MAX_PARTIALS) grid = B2_MAX_PARTIALS;
-    b2_join_agg_kernel<3><<<grid, B2_BLOCK, 0, st>>>(*scan, probe_key, *jt, ja, partials);
-  }
+  int grid = b2_wave_grid(b2_join_agg_kernel, B2_BLOCK, nblk);
+  if (grid > B2_MAX_PARTIALS) grid = B2_MAX_PARTIALS;
+  b2_join_agg_kernel<<<grid, B2_BLOCK, 0, st>>>(*scan, probe_key, *jt, ja, partials);
   B2_CHECK_LAUNCH("b2_join_agg_kernel");
   b2_scan_agg_final_kernel<<<naggs, B2_BLOCK, 0, st>>>(fa, partials, grid, d_out_acc, d_out_cnt, accumulate);
   B2_CHECK_LAUNCH("b2_scan_agg_final_kernel");

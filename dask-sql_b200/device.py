@@ -664,12 +664,13 @@ def join_probe_gather(scan, probe_keys, jt: JoinTable, mode, device, scan_cols, 
 def join_probe_onepass(scan, probe_keys, jt: JoinTable, mode, device, scan_cols, probe_gather, build_cols,
                        build_nullable):
     """join_probe_gather for direct-address tables without the counting pass and without the host
-    round trip: one kernel (b2_join_onepass: tile offsets by decoupled look-back), outputs allocated
-    at their upper bound (one row per probe row), the row count stays on the device.
-    -> (probe outputs, build outputs, 1-element int64 count tensor); slice with `trim` once known."""
+    round trip: one kernel (b2_join_onepass: each warp batch or tile reserves its output range with
+    an atomic, so rows come in probe order within a batch and in unspecified order across batches),
+    outputs allocated at their upper bound (one row per probe row), the row count stays on the device.
+    -> (trim, 1-element int64 count tensor); `trim(total)` slices the probe and build outputs."""
     assert jt.dense
     n = scan.n
-    ws = torch.zeros(L.join_onepass_ws_bytes(n) // 8, dtype=torch.int64, device=device)   # [total, status words]
+    total = torch.zeros(1, dtype=torch.int64, device=device)
     pk = (C.c_int32 * len(probe_keys))(*probe_keys)
     pouts, pvalid, bouts, bvalid = [], [], [], []
     for sl in probe_gather:
@@ -693,15 +694,8 @@ def join_probe_onepass(scan, probe_keys, jt: JoinTable, mode, device, scan_cols,
     else:
         bc = (L.Col * max(1, nb))(*[c.as_struct() for c in build_cols])
         bb = None
-    # offsets of the output rows: "stream" (default) = one launch, every warp batch reserves its range with an
-    # atomic, row order across batches unspecified (as SQL leaves it); "counted" = count + scan + write, output
-    # in probe order; "lookback" = one launch, probe order, offsets by decoupled look-back (measured slower)
-    order = os.environ.get("B200SQL_JOIN_ORDER", "stream")
-    if os.environ.get("B200SQL_JOIN_LOOKBACK") == "1":
-        order = "lookback"
-    lookback = {"stream": 2, "lookback": 1}.get(order, 0)
-    L.join_onepass(C.byref(scan), pk, C.byref(jt.struct), mode, lookback, ptr(ws), np_, pc, po, pv, nb, bc, bb,
-                   bo, bv, stream_ptr())
+    L.join_onepass(C.byref(scan), pk, C.byref(jt.struct), mode, ptr(total), np_, pc, po, pv, nb, bc, bb, bo, bv,
+                   stream_ptr())
 
     def trim(total):
         w = bitmap_words(total)
@@ -711,7 +705,7 @@ def join_probe_onepass(scan, probe_keys, jt: JoinTable, mode, device, scan_cols,
                 for o, v, c in zip(bouts, bvalid, build_cols)]
         return pres, bres
 
-    return trim, ws[:1]
+    return trim, total
 
 
 def join_probe(scan, probe_keys, jt: JoinTable, mode, device, build_matched=None):

@@ -2459,7 +2459,7 @@ def run_join(js: JoinSource, needed: Set[str]) -> List[Part]:
         kslots = [ctx.slot(e) for e in pk_exprs]
         refs = prefs
         if fused_gather and jt.dense and build_matched is None and os.environ.get("B200SQL_NO_ONEPASS") != "1":
-            # direct-address table: single-pass probe (look-back offsets), row count left on the device
+            # direct-address table: single-pass probe (offsets by atomic reservation), row count left on the device
             rslots = [ctx.slot(ColRef(r, part[r].dtype)) for r in refs]
             stats["launches"] += 3
             ev = _kernel_event_begin("b2_join_onepass", part.n)

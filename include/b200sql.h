@@ -493,18 +493,16 @@ int32_t b2_join_write_gather_keyed(const b2_scan_t* scan, const int32_t* probe_k
                                    uint32_t* const* build_valid, void* stream);
 
 /* Probe of a direct-address table (jt->dense 1 or 2; every probe row emits at most one output row in
- * all four modes) WITHOUT a host round trip: outputs are caller-allocated at their upper bound
- * (scan.n rows) and filled in probe-row order, the row count stays on the device.
- *   lookback == 0: count (key + presence only) -> scan -> write, three launches on `stream`;
- *   lookback != 0: one launch; each 2048-row tile learns its offset by a decoupled look-back over
- *                  the tiles before it (reads every input byte exactly once).
- * The write kernel front-loads its loads (key + first probe column, then presence word + the first
- * key-ordered payload speculatively), i.e. two dependent memory round trips per tile.
- * d_ws: b2_join_onepass_ws_bytes(n) bytes, ZEROED by the caller; its first int64 receives the number
- * of rows emitted.  Gather arguments as for b2_join_write_gather_keyed. */
-int64_t b2_join_onepass_ws_bytes(int64_t n);
+ * all four modes) in one launch, WITHOUT a host round trip: outputs are caller-allocated at their upper
+ * bound (scan.n rows), the row count stays on the device.  Rows of one 256-row warp batch (of one
+ * 2048-row tile when the specialised streaming kernel takes the shape) are contiguous and in probe
+ * order; the order of the batches themselves is unspecified.  The kernel front-loads its loads (key +
+ * first probe column, then presence word + the first key-ordered payload speculatively), i.e. two
+ * dependent memory round trips per batch.
+ * d_total: one int64, ZEROED by the caller; receives the number of rows emitted.  Gather arguments as
+ * for b2_join_write_gather_keyed. */
 int32_t b2_join_onepass(const b2_scan_t* scan, const int32_t* probe_keys, const b2_jointable_t* jt, int32_t mode,
-                        int32_t lookback, void* d_ws, int32_t nprobe, const int32_t* probe_cols,
+                        int64_t* d_total, int32_t nprobe, const int32_t* probe_cols,
                         void* const* probe_out, uint32_t* const* probe_valid, int32_t nbuild,
                         const b2_col_t* build_cols, const int64_t* build_base, void* const* build_out,
                         uint32_t* const* build_valid, void* stream);

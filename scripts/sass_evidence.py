@@ -12,7 +12,7 @@ LIB = os.path.join(ROOT, "dask-sql_b200", "libb200sql.so")
 OUT = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "build", "sass")
 WANT = {
     "star_agg": r"b2_star_agg_kernel",
-    "join_stream": r"b2_join_stream_kernelILb1ELi3ELb1ELb1E",
+    "join_stream": r"b2_join_stream_kernelILb1ELi3ELb1EE",
     "join_agg_fast": r"b2_join_agg_fast_kernelILb1ELi0E",
     "part_scatter_block": r"b2_part_scatter_kernel",
     "peer_merge_w8": r"b2_peer_merge_kernelILi8E",

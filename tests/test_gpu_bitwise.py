@@ -267,8 +267,7 @@ def test_bitwise_star_agg(n):
 def test_bitwise_join_agg(n):
     """AND / OR / XOR of P, B and the int combinations P*B, P+B, P-B, B-P (I64, U32 + base, sentinel U32
     payloads), two partitions combined with accumulate = 1; the fast kernel is SUM-only, so every case runs the
-    generic kernel and its 2-CTA instance"""
-    from tests.test_gpu_groupagg import env
+    generic kernel"""
     rng = np.random.default_rng(8000 + n)
     bs = build_side(rng)
     facts = [probe_part(n, rng), probe_part(n // 2 + 1, rng)]
@@ -277,10 +276,8 @@ def test_bitwise_join_agg(n):
             aggs = [(pc, bc, comb, op) for op in (AND, OR, XOR)] + [(pc, bc, comb, COUNT), (-1, -1, G.JA_ROWS, COUNT)]
             for terms in ([], PRED):
                 exp = join_agg_expected(facts, terms, 1, bs, BUILD, aggs)
-                for sw in ({}, {"B200SQL_JA_MINB": 2}):
-                    with env(**sw):
-                        got = run_join_agg(facts, terms, 1, bs, BUILD, aggs)
-                    check_global(*got, exp, True, f"join_agg c{comb} p{pc} b{bc} {sw} terms={terms}")
+                got = run_join_agg(facts, terms, 1, bs, BUILD, aggs)
+                check_global(*got, exp, True, f"join_agg c{comb} p{pc} b{bc} terms={terms}")
 
 
 @pytest.mark.parametrize("n", [0, 1, 33, 4097, 8229, 100_003])

@@ -347,13 +347,13 @@ def test_dense_result_is_pending_until_used():
 
 
 @pytest.mark.parametrize("how", ["inner", "left", "leftsemi", "leftanti"])
-@pytest.mark.parametrize("order", ["counted", "stream"])
-def test_join_key_ordered_payload_layout(how, order, monkeypatch):
+@pytest.mark.parametrize("fk_nulls", [True, False])
+def test_join_key_ordered_payload_layout(how, fk_nulls, monkeypatch):
     """Unique dense build keys: build columns are re-laid in key order (narrow uint32 offsets for
-    small-range ints, 8 bytes otherwise, bool, nullable) and probed by key offset.  order=stream runs
-    the generic single-pass kernel with atomically reserved output ranges (nullable key, many columns)."""
+    small-range ints, 8 bytes otherwise, bool, nullable) and probed by key offset, with and without NULL
+    probe keys.  The result must hold the rows of the row-lookup table's and the oracle's; row order across
+    output batches is unspecified, so they are compared sorted."""
     from dask_sql_b200 import executor
-    monkeypatch.setenv("B200SQL_JOIN_ORDER", order)
     rng = np.random.default_rng(31)
     nd, nf = 20_000, 150_003
     pk = rng.permutation(nd * 2)[:nd].astype(np.int64) - 777           # unique, with holes, negative kmin
@@ -366,7 +366,8 @@ def test_join_key_ordered_payload_layout(how, order, monkeypatch):
         "ni": pd.array(np.where(rng.random(nd) < 0.2, None, rng.integers(0, 9, nd)), dtype="Int64"),
     })
     fk = rng.integers(-2000, nd * 2 + 500, nf).astype(np.int64)         # some outside [kmin, kmax], some in holes
-    fact = pd.DataFrame({"fk": pd.array(np.where(rng.random(nf) < 0.05, None, fk), dtype="Int64"),
+    nulls = rng.random(nf) < 0.05
+    fact = pd.DataFrame({"fk": pd.array(np.where(nulls, None, fk), dtype="Int64") if fk_nulls else fk,
                          "v": rng.random(nf)})
     f, d = _table(fact, 3), _table(dim)
     before = executor.stats["keyed_join"]
@@ -375,11 +376,7 @@ def test_join_key_ordered_payload_layout(how, order, monkeypatch):
     monkeypatch.setenv("B200SQL_NO_KEY_LAYOUT", "1")
     plain = f.merge(d, left_on=["fk"], right_on=["pk"], how=how).compute()
     assert executor.stats["keyed_join"] == before + 1
-    if order == "counted":
-        pd.testing.assert_frame_equal(got, plain)                        # same rows, same order, same dtypes
-    else:
-        assert list(got.dtypes) == list(plain.dtypes)
-        assert_frames(got, plain, sort_by=["fk", "v"])
+    pd.testing.assert_frame_equal(_sorted(got), _sorted(plain))          # same rows, same dtypes
     from oracle import pandas_oracle as O
     exp = O.join_on_columns(fact, dim, ["fk"], ["pk"], how)
     assert_frames(got[list(exp.columns)], exp, sort_by=["fk", "v"])
@@ -387,10 +384,10 @@ def test_join_key_ordered_payload_layout(how, order, monkeypatch):
 
 @pytest.mark.parametrize("how", ["inner", "left", "leftsemi", "leftanti"])
 @pytest.mark.parametrize("match", [0.03, 0.8])
-def test_join_single_pass_lookback_equals_two_pass(how, match, monkeypatch):
-    """b2_join_onepass (tile offsets by decoupled look-back, count left on the device) must emit
-    exactly the rows, in exactly the order, of the count + write protocol -- across many tiles,
-    with tiles that emit nothing and with a pushed-down probe filter."""
+def test_join_single_pass_equals_two_pass(how, match, monkeypatch):
+    """b2_join_onepass (output ranges reserved atomically, count left on the device) must emit
+    exactly the rows of the count + write protocol -- across many tiles, with tiles that emit
+    nothing and with a pushed-down probe filter.  Row order across batches is unspecified."""
     from dask_sql_b200 import executor
     rng = np.random.default_rng(int(match * 100) + 41)
     nd, nf = 50_000, 700_003
@@ -408,24 +405,14 @@ def test_join_single_pass_lookback_equals_two_pass(how, match, monkeypatch):
 
     from oracle import pandas_oracle as O
     exp = O.join_on_columns(fact[fact["x"] > -3], dim, ["fk"], ["pk"], how)
-    # default: streaming single pass (row order across warp batches unspecified) -> compare as multisets
     parts, streamed = run()
     assert all(isinstance(p, executor.PendingPart) for p in parts)
-    assert len(streamed) == len(exp)
-    assert_frames(streamed[list(exp.columns)], exp, sort_by=["fk", "v"])
-    # the two probe-order protocols must agree row for row
-    monkeypatch.setenv("B200SQL_JOIN_ORDER", "counted")
-    parts, got = run()
-    assert all(isinstance(p, executor.PendingPart) for p in parts)
-    monkeypatch.setenv("B200SQL_JOIN_ORDER", "lookback")
-    _, got_lb = run()
-    pd.testing.assert_frame_equal(got, got_lb)
     monkeypatch.setenv("B200SQL_NO_ONEPASS", "1")
     parts2, two_pass = run()
     assert not any(isinstance(p, executor.PendingPart) for p in parts2)
-    pd.testing.assert_frame_equal(got, two_pass)
-    assert len(got) == len(exp)
-    assert_frames(got[list(exp.columns)], exp, sort_by=["fk", "v"])
+    pd.testing.assert_frame_equal(_sorted(streamed), _sorted(two_pass))
+    assert len(streamed) == len(exp)
+    assert_frames(streamed[list(exp.columns)], exp, sort_by=["fk", "v"])
 
 
 @pytest.mark.parametrize("nullable_key", [False, True])

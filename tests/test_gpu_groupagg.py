@@ -1008,13 +1008,12 @@ def _ja_cases():
 @pytest.mark.parametrize("n", [0, 33, 4097, 100_003])
 def test_join_agg(n):
     """P, B, P*B, P+B, P-B, B-P and COUNT(*) with SUM / SUMF / MIN / MAX / COUNT over I64, F64, U32 + base and
-    sentinel U32 payloads, each through the fast kernel (where the shape allows it), the generic kernel and
-    its 2-CTA instance; two partitions combined with accumulate = 1"""
+    sentinel U32 payloads, each through the fast kernel (where the shape allows it) and the generic kernel; two
+    partitions combined with accumulate = 1"""
     rng = np.random.default_rng(900 + n)
     bs = build_side(rng)
     facts = [probe_part(n, rng), probe_part(n // 2 + 1, rng)]
-    modes = {"default": {}, "generic": {"B200SQL_JA_GENERIC": 1},
-             "minb2": {"B200SQL_JA_GENERIC": 1, "B200SQL_JA_MINB": 2}}
+    modes = {"default": {}, "generic": {"B200SQL_JA_GENERIC": 1}}
     for name, key_col, aggs, dyadic in _ja_cases():
         for terms in ([], PRED):
             exp = join_agg_expected(facts, terms, key_col, bs, BUILD, aggs)

@@ -1,12 +1,14 @@
 """The join kernels row for row against the NumPy reference of tests/join_ref.py, through the C-ABI:
 b2_join_build (chain invariants), b2_join_build_dense, b2_join_key_layout, the two-pass probe b2_join_count +
 b2_join_write / _write_gather / _write_gather_keyed over chained, direct-address and key-ordered tables, and
-b2_join_onepass in its counted, look-back and streaming forms -- every instance of the specialised streaming
-kernel under both B200SQL_JOIN_RESERVE settings, and every shape that falls back to the generic kernel.
+b2_join_onepass -- every instance of the specialised streaming kernel and every shape that falls back to the
+generic kernel.
 
 Probe indices, tile offsets, gathered words and validity words are compared exactly; the build rows of one
 probe row form a run whose order is unspecified (chains are built with atomicExch), so runs are compared as
-sets and every gathered build value against the build index emitted beside it.  Outputs start as garbage:
+sets and every gathered build value against the build index emitted beside it.  The single-pass probe leaves
+the order of its output batches unspecified: its rows are compared exactly after sorting by the gathered row
+id, or as a multiset where no row id is gathered.  Outputs start as garbage:
 rows past the emitted count must keep it and validity words past it must stay zero.  Row counts straddle the
 warp (32), the warp batch (256), the one-pass tile (2048) and the two-pass tile (4096), and one run per probe
 kernel is large enough (2112 x 4096 + 1 rows) for every grid-stride tile loop to wrap.
@@ -560,9 +562,11 @@ ONEPASS_CONFIGS = [
 ]
 
 
-def run_onepass(t, pcols, key_cols, terms, mode, lookback, pgi, bgi, with_valid, what, order="probe"):
-    """b2_join_onepass with outputs allocated at n rows of garbage; order "probe" compares row for row, "batch"
-    sorts by the gathered row id (which must be the first probe column) and checks the per-batch order"""
+def run_onepass(t, pcols, key_cols, terms, mode, pgi, bgi, with_valid, what, batch=256):
+    """b2_join_onepass with outputs allocated at n rows of garbage.  With the row id gathered the output is
+    sorted by it and compared exactly, and the rows of each `batch`-row probe batch must be contiguous and in
+    probe order; otherwise the rows, validity bits included, are compared as a multiset.  Rows past the total
+    keep their garbage and validity words hold no bit past it."""
     import torch
     L = _L()
     n = pcols[0].n
@@ -572,48 +576,47 @@ def run_onepass(t, pcols, key_cols, terms, mode, lookback, pgi, bgi, with_valid,
     e = J.emit(mode, passing, t.matches(pcols, passing, key_cols))
     pgc = [pcols[i] for i in pgi]
     bgc = [t.payload[i] for i in bgi if t.dense == 2 or i < 4] if mode in (J.JOIN_INNER, J.JOIN_LEFT) else []
-    flags = _u32_flags(t, bgc)
     pg = Gathered([_out_dtype(c) for c in pgc], n, with_valid)
     bg = Gathered([_out_dtype(c) for c in bgc], n, with_valid)
     keep = []
-    bcols = col_array(bgc, keep, flags)
-    base = (C.c_int64 * max(1, len(bgc)))(*[getattr(t, "u32_base", 0)] * len(bgc))
-    ws = torch.zeros(L.join_onepass_ws_bytes(n) // 8 + 1, dtype=torch.int64, device=_dev())
+    bcols = col_array(bgc, keep, _u32_flags(t, bgc))
+    u32_base = getattr(t, "u32_base", 0)
+    base = (C.c_int64 * max(1, len(bgc)))(*[u32_base] * len(bgc))
+    count = torch.zeros(1, dtype=torch.int64, device=_dev())
     pc = (C.c_int32 * max(1, len(pgc)))(*list(pgi))
-    L.join_onepass(C.byref(scan), pk, C.byref(t.jt), mode, lookback, _ptr(ws), len(pgc), pc, pg.out, pg.vptr(),
+    L.join_onepass(C.byref(scan), pk, C.byref(t.jt), mode, _ptr(count), len(pgc), pc, pg.out, pg.vptr(),
                    len(bgc), bcols, base, bg.out, bg.vptr(), _stream())
-    total = int(_np(ws)[0])
-    assert total == e.total, f"{what}: ws[0] = {total} rows, expected {e.total}"
-    if order == "probe":
-        perm = np.arange(total)
+    total = int(_np(count)[0])
+    assert total == e.total, f"{what}: {total} rows emitted, expected {e.total}"
+    exp = [J.gather_probe(c, e.probe) for c in pgc] + [J.gather_build(c, e.build, u32_base) for c in bgc]
+    outs = [(pg, k) for k in range(len(pgc))] + [(bg, k) for k in range(len(bgc))]
+    got, want = [], []     # one field per output column and one per validity output beside it
+    for i, ((g, k), (vals, valid)) in enumerate(zip(outs, exp)):
+        d = _np(g.data[k])
+        fill = 0x5A if g.dtypes[k] == R.U8 else GARBAGE
+        _assert_words(d[total:], np.full(len(d) - total, fill, d.dtype), f"{what}: column {i} past the total")
+        got.append(d[:total].astype(np.int64))
+        want.append(np.asarray(vals, d.dtype).astype(np.int64))
+        if g.valid[k] is not None:
+            w = _np(g.valid[k]).view(np.uint32)
+            r = np.arange(total)
+            bits = ((w[r >> 5] >> (r & 31)) & 1).astype(np.int64)
+            _assert_words(w, J.valid_words(bits, len(w)), f"{what}: column {i} validity words past the total")
+            got.append(bits)
+            want.append(np.asarray(valid, np.int64))
+    gs = np.stack(got, axis=1) if got else np.zeros((total, 0), np.int64)
+    xs = np.stack(want, axis=1) if want else np.zeros((total, 0), np.int64)
+    if PID in pgi:
+        pid = _np(pg.data[list(pgi).index(PID)])[:total]
+        check_batch_order(pid, batch, what)
+        gs = gs[np.argsort(pid, kind="stable")]
+        how = "sorted by row id"
     else:
-        got_pid = _np(pg.data[0])[:total]
-        batch = 2048 if order == "tile" else 256
-        check_batch_order(got_pid, batch, what)
-        perm = np.argsort(got_pid, kind="stable")
-    for k, c in enumerate(pgc):
-        vals, valid = J.gather_probe(c, e.probe)
-        check_permuted(pg, k, total, perm, vals, valid, f"{what}: probe")
-    for k, c in enumerate(bgc):
-        vals, valid = J.gather_build(c, e.build, getattr(t, "u32_base", 0))
-        check_permuted(bg, k, total, perm, vals, valid, f"{what}: build")
-    return pg, bg, total
-
-
-def check_permuted(g: Gathered, k, total, perm, vals, valid, what):
-    """output column k, read in the order `perm`, against the reference; rows past the total unchanged"""
-    got = _np(g.data[k])
-    inv = np.empty_like(perm)
-    inv[perm] = np.arange(len(perm))
-    u8 = g.dtypes[k] == R.U8
-    exp = np.asarray(vals, got.dtype)
-    _assert_words(got[:total][perm], exp, f"{what}: column {k} values")
-    _assert_words(got[total:], np.full(len(got) - total, 0x5A if u8 else GARBAGE, got.dtype),
-                  f"{what}: column {k} rows past the {total} emitted")
-    if g.valid[k] is not None:
-        w = _np(g.valid[k]).view(np.uint32)
-        v = np.asarray(valid, bool)[inv] if total else np.zeros(0, bool)
-        _assert_words(w, J.valid_words(v, len(w)), f"{what}: column {k} validity words")
+        if gs.size:
+            gs, xs = gs[np.lexsort(gs.T[::-1])], xs[np.lexsort(xs.T[::-1])]
+        how = "as a multiset of rows"
+    for i in range(gs.shape[1]):
+        _assert_words(gs[:, i], xs[:, i], f"{what}: field {i}, {how}")
 
 
 def check_batch_order(pid, batch, what):
@@ -629,106 +632,61 @@ def check_batch_order(pid, batch, what):
 
 
 @pytest.mark.parametrize("n", SIZES)
-@pytest.mark.parametrize("lookback", [0, 1])
+@pytest.mark.parametrize("mode", MODES, ids=["inner", "left", "semi", "anti"])
 @pytest.mark.parametrize("dense", [1, 2])
-def test_join_onepass_ordered(dense, lookback, n):
-    """counted (lookback 0) and decoupled look-back (1) probes of direct-address and key-ordered tables: row for
-    row in probe order in all four modes, ws[0] the total, garbage past it untouched"""
+def test_join_onepass_ordered(dense, mode, n):
+    """the generic single-pass kernel (a nullable key never takes the streaming one) over direct-address and
+    key-ordered tables: each 256-row warp batch's rows contiguous and in probe order, every row exact, the total
+    and garbage past it untouched"""
     rng = np.random.default_rng(500 + n)
     t, pcols, key_cols = make_table("dense1" if dense == 1 else "dense2", n, rng)
     for terms in (T_NONE, T_OTHER, t_key(_kmid(pcols))):
-        for mode in MODES:
-            for pgi, bgi, wv in ONEPASS_CONFIGS:
-                run_onepass(t, pcols, key_cols, terms, mode, lookback, pgi, bgi, wv,
-                            f"dense={dense} lookback={lookback} n={n} mode={mode} terms={terms} probe={pgi}")
+        for pgi, bgi, wv in ONEPASS_CONFIGS:
+            run_onepass(t, pcols, key_cols, terms, mode, pgi, bgi, wv,
+                        f"dense={dense} n={n} mode={mode} terms={terms} probe={pgi}")
 
 
-# the 30 launchable instances of b2_join_stream_kernel<HAS_P, BMODE, OUT_KEY, CTA_RES>, per reservation
+# the 15 launchable instances of b2_join_stream_kernel<HAS_P, BMODE, OUT_KEY>
 STREAM_INSTANCES = [(hp, bm, ok) for hp in (False, True) for bm in range(4) for ok in (False, True)
                     if hp or bm or ok]
 STREAM_PAYLOAD = {1: 0, 2: 4, 3: 5}     # BMODE -> key-ordered payload: I64 row id, U32 + base, U32 sentinel
 
 
-def run_stream(t, pcols, terms, mode, pgi, bgi, what, tile_order):
-    """b2_join_onepass(lookback = 2); with the row id gathered (first probe column) the output is sorted by it
-    and compared exactly, otherwise compared as a multiset of rows"""
-    import torch
-    L = _L()
-    n = pcols[0].n
-    scan = scan_of(pcols, terms)
-    pk = (C.c_int32 * 1)(KN)
-    passing = R.eval_terms(pcols, terms, n)
-    e = J.emit(mode, passing, t.matches(pcols, passing, [KN]))
-    pgc = [pcols[i] for i in pgi]
-    bgc = [t.payload[i] for i in bgi]
-    pg = Gathered([R.I64] * len(pgc), n, False)
-    bg = Gathered([_out_dtype(c) for c in bgc], n, False)
-    keep = []
-    bcols = col_array(bgc, keep, _u32_flags(t, bgc))
-    base = (C.c_int64 * max(1, len(bgc)))(*[t.u32_base] * len(bgc))
-    ws = torch.zeros(L.join_onepass_ws_bytes(n) // 8 + 1, dtype=torch.int64, device=_dev())
-    pc = (C.c_int32 * max(1, len(pgc)))(*list(pgi))
-    L.join_onepass(C.byref(scan), pk, C.byref(t.jt), mode, 2, _ptr(ws), len(pgc), pc, pg.out, None, len(bgc), bcols,
-                   base, bg.out, None, _stream())
-    total = int(_np(ws)[0])
-    assert total == e.total, f"{what}: ws[0] = {total} rows, expected {e.total}"
-    exp = [J.gather_probe(c, e.probe)[0] for c in pgc] + [J.gather_build(c, e.build, t.u32_base)[0] for c in bgc]
-    got = [_np(x) for x in pg.data + bg.data]
-    for k, g in enumerate(got):
-        _assert_words(g[total:], np.full(len(g) - total, GARBAGE, g.dtype), f"{what}: column {k} past the total")
-    got = [g[:total] for g in got]
-    if pgi and pgi[0] == PID:
-        check_batch_order(got[0], 2048 if tile_order else 256, what)
-        perm = np.argsort(got[0], kind="stable")
-        for k, (g, x) in enumerate(zip(got, exp)):
-            _assert_words(g[perm], np.asarray(x, np.int64), f"{what}: column {k}")
-    else:
-        gs = np.stack(got, axis=1) if got else np.zeros((total, 0), np.int64)
-        xs = np.stack([np.asarray(x, np.int64) for x in exp], axis=1)
-        gs, xs = gs[np.lexsort(gs.T[::-1])] if len(gs) else gs, xs[np.lexsort(xs.T[::-1])] if len(xs) else xs
-        _assert_words(gs.reshape(-1), xs.reshape(-1), f"{what}: rows as a multiset")
-
-
 @pytest.mark.parametrize("n", SIZES)
-@pytest.mark.parametrize("reserve", ["cta", "warp"])
-def test_join_onepass_stream(reserve, n):
-    """lookback = 2 reaches every instance of the streaming kernel (extra probe column, build payload mode 0-3,
-    key output) under B200SQL_JOIN_RESERVE=cta / warp, and every shape that falls back to the generic kernel:
-    nullable key, U8 column, validity output, LEFT / ANTI, two build columns, three probe columns, a direct-address
-    (not key-ordered) table.  CTA reservation keeps each 2048-row tile's rows together and in probe order, warp
-    reservation and the generic kernel each 256-row warp batch's."""
+@pytest.mark.parametrize("terms", [T_NONE, T_OTHER], ids=["no_terms", "term"])
+def test_join_onepass_stream(terms, n):
+    """every instance of the streaming kernel (extra probe column, build payload mode 0-3, key output), which
+    keeps each 2048-row tile's rows together and in probe order, and every shape that falls back to the generic
+    kernel, which keeps each 256-row warp batch's: nullable key, U8 column, validity output, LEFT / ANTI, two
+    build columns, three probe columns, a direct-address (not key-ordered) table"""
     rng = np.random.default_rng(600 + n)
     t, pcols, _ = make_table("dense2", n, rng)
     t1, p1, _ = make_table("dense1", n, rng)
-    with env(B200SQL_JOIN_RESERVE=reserve):
-        for terms in (T_NONE, T_OTHER):
-            for hp, bm, ok in STREAM_INSTANCES:
-                pgi = ([PID] if hp else []) + ([KN] if ok else [])
-                bgi = [STREAM_PAYLOAD[bm]] if bm else []
-                for mode in (J.JOIN_INNER, J.JOIN_SEMI) if not bm else (J.JOIN_INNER,):
-                    run_stream(t, pcols, terms, mode, pgi, bgi,
-                               f"stream {reserve} n={n} hp={hp} bmode={bm} key={ok} mode={mode} terms={terms}",
-                               reserve == "cta")
-            # fallbacks to the generic kernel (one atomic per warp batch): row id first, so sorted compare
-            what = f"generic {reserve} n={n} terms={terms}"
-            for name, key_cols, pgi, bgi, mode, wv in [
-                    ("nullable key", [K0], (PID,), (0,), J.JOIN_INNER, False),
-                    ("U8 probe column", [KN], (PID, PU), (0,), J.JOIN_INNER, False),
-                    ("U8 build column", [KN], (PID,), (2,), J.JOIN_INNER, False),
-                    ("validity output", [KN], (PID, KN), (4,), J.JOIN_INNER, True),
-                    ("LEFT", [KN], (PID, KN), (0,), J.JOIN_LEFT, False),
-                    ("ANTI", [KN], (PID,), (), J.JOIN_ANTI, False),
-                    ("two build columns", [KN], (PID,), (0, 4), J.JOIN_INNER, False),
-                    ("three probe columns", [KN], (PID, KN, P), (5,), J.JOIN_INNER, False)]:
-                run_onepass(t, pcols, key_cols, terms, mode, 2, pgi, bgi, wv, f"{what} {name}", order="batch")
-            run_onepass(t1, p1, [KN], terms, J.JOIN_INNER, 2, (PID, KN), (0,), False, f"{what} dense 1", order="batch")
+    for hp, bm, ok in STREAM_INSTANCES:
+        pgi = ([PID] if hp else []) + ([KN] if ok else [])
+        bgi = [STREAM_PAYLOAD[bm]] if bm else []
+        for mode in (J.JOIN_INNER, J.JOIN_SEMI) if not bm else (J.JOIN_INNER,):
+            run_onepass(t, pcols, [KN], terms, mode, pgi, bgi, False,
+                        f"stream n={n} hp={hp} bmode={bm} key={ok} mode={mode} terms={terms}", batch=2048)
+    what = f"generic n={n} terms={terms}"
+    for name, key_cols, pgi, bgi, mode, wv in [
+            ("nullable key", [K0], (PID,), (0,), J.JOIN_INNER, False),
+            ("U8 probe column", [KN], (PID, PU), (0,), J.JOIN_INNER, False),
+            ("U8 build column", [KN], (PID,), (2,), J.JOIN_INNER, False),
+            ("validity output", [KN], (PID, KN), (4,), J.JOIN_INNER, True),
+            ("LEFT", [KN], (PID, KN), (0,), J.JOIN_LEFT, False),
+            ("ANTI", [KN], (PID,), (), J.JOIN_ANTI, False),
+            ("two build columns", [KN], (PID,), (0, 4), J.JOIN_INNER, False),
+            ("three probe columns", [KN], (PID, KN, P), (5,), J.JOIN_INNER, False)]:
+        run_onepass(t, pcols, key_cols, terms, mode, pgi, bgi, wv, f"{what} {name}")
+    run_onepass(t1, p1, [KN], terms, J.JOIN_INNER, (PID, KN), (0,), False, f"{what} dense 1")
 
 
 # ---- one run per probe kernel with wrapping tile loops -------------------------------------------------------------
 def test_join_probes_wrap_their_tile_loops():
-    """2112 x 4096 + 1 probe rows: more than two waves of resident blocks for 4096- and 2048-row tiles, look-back
-    over more than 32 predecessors and a partial last tile, for the two-pass probe (chained and direct-address),
-    the counted and look-back one-pass probes, the streaming kernel under both reservations and the generic one"""
+    """2112 x 4096 + 1 probe rows: more than two waves of resident blocks for 4096- and 2048-row tiles and a
+    partial last tile, for the two-pass probe (chained and direct-address), the generic single-pass kernel and
+    the streaming one"""
     n = BIG_N
     rng = np.random.default_rng(700)
     for kind in ("chained", "dense1"):
@@ -742,13 +700,8 @@ def test_join_probes_wrap_their_tile_loops():
         run_two_pass_big(t, pcols, kind)
     t = direct_table(2, 40_000, rng, -1000)
     pcols = probe_cols(n, rng, direct_probe_keys(n, t, rng))
-    for lookback in (0, 1):
-        run_onepass(t, pcols, [K0], T_OTHER, J.JOIN_LEFT, lookback, (PID, PF), (4, 1), True,
-                    f"big onepass lookback={lookback}")
-    for reserve in ("cta", "warp"):
-        with env(B200SQL_JOIN_RESERVE=reserve):
-            run_stream(t, pcols, T_OTHER, J.JOIN_INNER, [PID, KN], [4], f"big stream {reserve}", reserve == "cta")
-    run_onepass(t, pcols, [K0], T_OTHER, J.JOIN_INNER, 2, (PID,), (0,), False, "big generic", order="batch")
+    run_onepass(t, pcols, [K0], T_OTHER, J.JOIN_LEFT, (PID, PF), (4, 1), True, "big generic")
+    run_onepass(t, pcols, [KN], T_OTHER, J.JOIN_INNER, [PID, KN], [4], False, "big stream", batch=2048)
 
 
 def run_two_pass_big(t, pcols, kind):
@@ -803,7 +756,7 @@ class ArgCase:
         self.outp = _zeros(n)
         self.outb = _zeros(n)
         self.matched = _zeros(4 * n, torch.uint8)
-        self.ws = torch.zeros(L.join_onepass_ws_bytes(n) // 8 + 1, dtype=torch.int64, device=_dev())
+        self.count = _zeros(1, torch.int64)
         self.gout = _zeros(4 * n, torch.int64)
         self.gval = _zeros(n)
         self.bcol = col_struct(R.Column(np.arange(4 * n, dtype=np.int64), None, R.I64), self.keep)
@@ -847,8 +800,8 @@ class ArgCase:
             s, pk, C.byref(jt), mode, _ptr(self.off), _ptr(self.outp), _ptr(self.outb), mp, nprobe, gcols, gout, gval,
             nbuild, bcols, base, gout, gval, st)
         if jt.dense and not matched:
-            self.ws.zero_()
-            rcs["onepass"] = lib.b2_join_onepass(s, pk, C.byref(jt), mode, 1, _ptr(self.ws), nprobe, gcols, gout, gval,
+            self.count.zero_()
+            rcs["onepass"] = lib.b2_join_onepass(s, pk, C.byref(jt), mode, _ptr(self.count), nprobe, gcols, gout, gval,
                                                  nbuild, bcols, base, gout, gval, st)
         _np(self.off)
         return rcs
