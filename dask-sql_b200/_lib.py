@@ -89,6 +89,7 @@ class StarLookup(C.Structure):
 
 
 MAX_PEERS, PEER_MAX_ARRAYS = 16, 2 * MAX_AGGS + 1
+STAR_MAX_PARTS = 16                  # partitions per b2_star_agg_multi launch (include/b200sql.h)
 PEER_SUM_F64, PEER_SUM_I64, PEER_MIN_I64, PEER_MAX_I64, PEER_AND_I64, PEER_OR_I64, PEER_XOR_I64 = range(7)
 PEER_PRESENT_ROWS, PEER_PRESENT_INDICATOR, PEER_PRESENT_BITMAP = 1, 2, 3
 
@@ -212,6 +213,9 @@ _SIGS = {
                                   C.c_int32, _P, _P, C.c_int32, _P],
     "b2_star_agg_narrow": [C.POINTER(Scan), _P, C.c_int32, C.POINTER(StarLookup), C.POINTER(Agg), C.c_int32,
                            C.POINTER(AggState), _P],
+    "b2_star_agg_multi": [C.POINTER(Scan), _P, C.c_int32, C.c_int32, C.POINTER(StarLookup), C.POINTER(Agg), C.c_int32,
+                          C.POINTER(AggState), _P, _P],
+    "b2_star_build_pack": [_P, C.c_int64, _P, C.c_int64, _P, C.c_int32, _P],
     "b2_str_like": [_P, _P, C.c_int64, _P, C.c_int64, C.c_uint32, C.c_int32, _P, _P],
     "b2_str_lower_bound": [_P, _P, C.c_int64, _P, _P, C.c_int64, C.c_int32, _P, _P, _P],
 }
@@ -307,6 +311,8 @@ star_agg = _wrap("b2_star_agg")
 star_build_mark_narrow = _wrap("b2_star_build_mark_narrow")
 star_build_fill_narrow = _wrap("b2_star_build_fill_narrow")
 star_agg_narrow = _wrap("b2_star_agg_narrow")
+star_agg_multi = _wrap("b2_star_agg_multi")
+star_build_pack = _wrap("b2_star_build_pack")
 str_like = _wrap("b2_str_like")
 str_lower_bound = _wrap("b2_str_lower_bound")
 num_tiles = _lib.b2_num_tiles

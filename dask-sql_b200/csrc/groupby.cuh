@@ -572,6 +572,72 @@ b2_star_agg_kernel(const __grid_constant__ b2_scan_narrow_t sn, int fk_col, cons
   b2_tile_direct<B2_STAR_R, true>(s, [&](const b2_gld_t<true>& ld) { b2_star_body<B2_STAR_R>(s, ld, fk_col, lk, aggs, st); });
 }
 
+// The partitions of one b2_star_agg_multi launch, all in parameter space: the body reads a partition's scan
+// from the constant bank exactly as b2_star_agg_kernel reads its one scan.  Tiles of B2_BLOCK x B2_STAR_R
+// rows never cross a partition; partition p owns tiles [tile0[p], tile0[p + 1]).  Tiles [0, nstatic) are
+// strided over the CTAs as in b2_tile_direct (no ticket round trip), the rest are handed out by a ticket, so
+// that a CTA that runs ahead takes more of the tail and the grid ends together.
+struct b2_star_parts_arg {
+  b2_scan_narrow_t p[B2_STAR_MAX_PARTS];
+  int64_t tile0[B2_STAR_MAX_PARTS + 1];
+  int64_t nstatic;
+  int32_t nparts;
+};
+
+__global__ void __launch_bounds__(B2_BLOCK, 2)
+b2_star_agg_multi_kernel(const __grid_constant__ b2_star_parts_arg pa, int fk_col,
+                         const __grid_constant__ b2_starlookup_t lk, const __grid_constant__ b2_aggs_arg aggs,
+                         const __grid_constant__ b2_aggstate_t st, unsigned long long* __restrict__ ticket) {
+  __shared__ long long sh_tile[2];
+  const int tile_off = (threadIdx.x >> 5) * (32 * B2_STAR_R) + (threadIdx.x & 31);
+  const int64_t tile = (int64_t)B2_BLOCK * B2_STAR_R;
+  const int64_t ntiles = pa.tile0[pa.nparts];
+  // One call site of the body (a second inlined copy spills).  The ticket of the next tile is taken while
+  // the current one runs, into the other half of sh_tile; every CTA takes one ticket past the end.
+  auto take = [&](int k) {
+    if (threadIdx.x == 0) sh_tile[k] = pa.nstatic + (long long)atomicAdd(ticket, 1ULL);
+  };
+  int64_t t = blockIdx.x;
+  int k = 0;
+  if (t >= pa.nstatic) {
+    take(0);
+    __syncthreads();
+    t = sh_tile[0];
+  }
+  while (t < ntiles) {
+    const bool by_ticket = t + gridDim.x >= pa.nstatic;   // the next tile is not a static one: uniform in the CTA
+    if (by_ticket) take(k ^ 1);
+    int p = 0;
+    while (p + 1 < pa.nparts && pa.tile0[p + 1] <= t) ++p;   // skips empty partitions: tile0[p + 1] == tile0[p]
+    const b2_scan_t& s = pa.p[p].s;
+    const b2_gld_t<true> ld{&s, (t - pa.tile0[p]) * tile + tile_off};
+    b2_star_body<B2_STAR_R>(s, ld, fk_col, lk, aggs, st);
+    if (by_ticket) {
+      __syncthreads();
+      k ^= 1;
+      t = sh_tile[k];
+    } else {
+      t += gridDim.x;
+    }
+  }
+}
+
+// 21-bit slots packed from their int32 staging array (b2_star_build_pack): word q = entries 3q .. 3q + 2; the
+// entries past the last set bit of the directory were never stored, and are 0
+__global__ void __launch_bounds__(B2_BLOCK)
+b2_star_pack21_kernel(const uint64_t* __restrict__ dir, int64_t nwords, const int32_t* __restrict__ staged,
+                      int64_t nout, uint64_t* __restrict__ slots) {
+  const uint64_t last = dir[nwords - 1];
+  const int64_t nset = (int64_t)(last >> 32) + __popc((uint32_t)last);
+  for (int64_t q = (int64_t)blockIdx.x * B2_BLOCK + threadIdx.x; q < nout; q += (int64_t)gridDim.x * B2_BLOCK) {
+    uint64_t w = 0;
+#pragma unroll
+    for (int e = 0; e < 3; ++e)
+      if (3 * q + e < nset) w |= ((uint64_t)(uint32_t)staged[3 * q + e] & 0x1FFFFFull) << (21 * e);
+    slots[q] = w;
+  }
+}
+
 extern "C" {
 
 static int32_t b2_check_state(const b2_aggs_arg& aa, const b2_aggstate_t* st) {
@@ -870,6 +936,74 @@ int32_t b2_star_build_hash(const b2_col_t* pk, const int32_t* sel, int64_t n_sel
   return B2_OK;
 }
 
+// the lookup check of the star probes; *out is the kernel parameter (slot_bits 0 normalised to 32)
+static int32_t b2_check_starlookup(const b2_starlookup_t* lk, b2_starlookup_t* out) {
+  B2_REQUIRE(lk, "null lookup");
+  B2_REQUIRE(lk->dense >= 0 && lk->dense <= 2, "bad lookup kind");
+  b2_starlookup_t l = *lk;
+  if (l.dense == 2) {
+    B2_REQUIRE(l.dir && l.lookup && l.range > 0 && l.range < ((int64_t)1 << 31), "bad bitmap lookup");
+    if (l.slot_bits == 0) l.slot_bits = 32;
+    B2_REQUIRE(l.slot_bits == 16 || l.slot_bits == 21 || l.slot_bits == 32, "slot_bits must be 0, 16, 21 or 32");
+    B2_REQUIRE(l.slot_bits == 32 || ((uintptr_t)l.lookup & 7) == 0, "packed slots must be 8-byte aligned");
+  }
+  else if (l.dense) B2_REQUIRE(l.lookup && l.range > 0, "bad dense lookup");
+  else B2_REQUIRE(l.table_keys && l.table_slots && b2_pow2(l.cap), "bad hash lookup");
+  *out = l;
+  return B2_OK;
+}
+
+int32_t b2_star_build_pack(const uint64_t* dir, int64_t pk_range, const int32_t* staged, int64_t capacity,
+                           uint64_t* slots, int32_t slot_bits, void* stream) {
+  B2_REQUIRE(dir && staged && slots, "null argument");
+  B2_REQUIRE(slot_bits == 21, "only 21-bit slots are packed from a staging array");
+  B2_REQUIRE(pk_range > 0 && pk_range < ((int64_t)1 << 31), "bad range");
+  B2_REQUIRE(capacity >= 0 && capacity <= pk_range, "bad capacity");
+  const int64_t nout = (capacity + 2) / 3;
+  if (nout == 0) return B2_OK;
+  int grid = b2_wave_grid(b2_star_pack21_kernel, B2_BLOCK, (nout + B2_BLOCK - 1) / B2_BLOCK);
+  b2_star_pack21_kernel<<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(dir, (pk_range + 31) / 32, staged, nout, slots);
+  B2_CHECK_LAUNCH("b2_star_pack21_kernel");
+  return B2_OK;
+}
+
+int32_t b2_star_agg_multi(const b2_scan_t* scans, const int64_t* const* bases, int32_t nparts, int32_t fk_col,
+                          const b2_starlookup_t* lk, const b2_agg_t* aggs, int32_t naggs, const b2_aggstate_t* st,
+                          uint64_t* d_tickets, void* stream) {
+  B2_REQUIRE(scans && d_tickets && nparts >= 0, "null argument");
+  // out_slot is indexed by the row within a partition: with several partitions they would overwrite each other
+  B2_REQUIRE(!st || !st->out_slot || nparts <= 1, "out_slot needs a single partition");
+  b2_starlookup_t l;
+  int32_t rc = b2_check_starlookup(lk, &l);
+  if (rc) return rc;
+  b2_aggs_arg aa;
+  const int64_t tile = (int64_t)B2_BLOCK * B2_STAR_R;
+  for (int32_t first = 0, launch = 0; first < nparts; first += B2_STAR_MAX_PARTS, ++launch) {
+    static thread_local b2_star_parts_arg pa;   // 13 KB: not on the caller's stack; the launch copies it
+    memset(&pa, 0, sizeof(pa));
+    pa.nparts = nparts - first < B2_STAR_MAX_PARTS ? nparts - first : B2_STAR_MAX_PARTS;
+    for (int p = 0; p < pa.nparts; ++p) {
+      const b2_scan_t* scan = scans + first + p;
+      if ((rc = b2_check_narrow_scan(scan, bases ? bases[first + p] : nullptr, &pa.p[p]))) return rc;
+      if ((rc = b2_check_aggs(scan, aggs, naggs, &aa))) return rc;
+      B2_REQUIRE(fk_col >= 0 && fk_col < scan->ncols, "fk column out of range");
+      B2_REQUIRE(b2_is_int64_scan_col(scan->cols[fk_col]), "fk must be int64");
+      pa.tile0[p + 1] = pa.tile0[p] + (scan->n + tile - 1) / tile;
+    }
+    if ((rc = b2_check_state(aa, st))) return rc;
+    const int64_t ntiles = pa.tile0[pa.nparts];
+    if (ntiles == 0) continue;
+    const int grid = b2_wave_grid(b2_star_agg_multi_kernel, B2_BLOCK, ntiles);
+    // 90 % static: on C4 (8 x 125M rows, H100) tickets for every tile or for the last 25 % measured the same
+    pa.nstatic = ntiles * 9 / 10 / grid * grid;
+    if (pa.nstatic > ntiles) pa.nstatic = ntiles;
+    b2_star_agg_multi_kernel<<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(
+        pa, fk_col, l, aa, *st, reinterpret_cast<unsigned long long*>(d_tickets) + launch);
+    B2_CHECK_LAUNCH("b2_star_agg_multi_kernel");
+  }
+  return B2_OK;
+}
+
 int32_t b2_star_agg(const b2_scan_t* scan, int32_t fk_col, const b2_starlookup_t* lk, const b2_agg_t* aggs,
                     int32_t naggs, const b2_aggstate_t* st, void* stream) {
   return b2_star_agg_narrow(scan, nullptr, fk_col, lk, aggs, naggs, st, stream);
@@ -883,19 +1017,10 @@ int32_t b2_star_agg_narrow(const b2_scan_t* scan, const int64_t* bases, int32_t 
   b2_aggs_arg aa;
   if ((rc = b2_check_aggs(scan, aggs, naggs, &aa))) return rc;
   if ((rc = b2_check_state(aa, st))) return rc;
-  B2_REQUIRE(lk, "null lookup");
   B2_REQUIRE(fk_col >= 0 && fk_col < scan->ncols, "fk column out of range");
   B2_REQUIRE(b2_is_int64_scan_col(scan->cols[fk_col]), "fk must be int64");
-  B2_REQUIRE(lk->dense >= 0 && lk->dense <= 2, "bad lookup kind");
-  b2_starlookup_t l = *lk;
-  if (l.dense == 2) {
-    B2_REQUIRE(l.dir && l.lookup && l.range > 0 && l.range < ((int64_t)1 << 31), "bad bitmap lookup");
-    if (l.slot_bits == 0) l.slot_bits = 32;
-    B2_REQUIRE(l.slot_bits == 16 || l.slot_bits == 21 || l.slot_bits == 32, "slot_bits must be 0, 16, 21 or 32");
-    B2_REQUIRE(l.slot_bits == 32 || ((uintptr_t)l.lookup & 7) == 0, "packed slots must be 8-byte aligned");
-  }
-  else if (l.dense) B2_REQUIRE(l.lookup && l.range > 0, "bad dense lookup");
-  else B2_REQUIRE(l.table_keys && l.table_slots && b2_pow2(l.cap), "bad hash lookup");
+  b2_starlookup_t l;
+  if ((rc = b2_check_starlookup(lk, &l))) return rc;
   if (scan->n == 0) return B2_OK;
   int64_t nblk = (scan->n + (int64_t)B2_BLOCK * B2_STAR_R - 1) / ((int64_t)B2_BLOCK * B2_STAR_R);
   int grid = b2_wave_grid(b2_star_agg_kernel, B2_BLOCK, nblk);

@@ -1730,15 +1730,27 @@ class PreparedStar:
             self.dim_launch.append(self._launch(ctx, pk_slot, g_slot))
             self.keep.append(ctx)
         self.fact_launch = []
+        fact_specs = set()
         for part in fparts:
             if part.n == 0:
                 continue
             ctx = ScanCtx(part, q.fpred)
             fk_slot = ctx.slot(q.fk_e)
             specs = [(ctx.slot(ka.expr), ka.op) for ka in q.plan.kaggs]
+            fact_specs.add((fk_slot, tuple(specs)))
             self._only_table_columns(ctx)
             self.fact_launch.append(self._launch(ctx, fk_slot, D.make_aggs(specs), len(specs), part.n))
             self.keep.append(ctx)
+        # One probe launch (b2_star_agg_multi) per L.STAR_MAX_PARTS fact partitions when their scans index the
+        # key and the aggregate inputs alike; B200SQL_STAR_PER_PART=1: one b2_star_agg launch per partition and
+        # the CAS fill of 21-bit slots, as before the multi-partition probe and the staged fill.
+        per_part = os.environ.get("B200SQL_STAR_PER_PART") == "1"
+        self.multi = not per_part and len(fact_specs) == 1
+        self.fact_rows = sum(launch[-1] for launch in self.fact_launch)
+        # the probe's tile tickets, one per launch: this rank's own, zeroed by every run before its probe, and never
+        # part of the broadcast lookup buffer, whose size all ranks agree on
+        self.tickets = torch.zeros(-(-len(self.fact_launch) // L.STAR_MAX_PARTS), dtype=torch.int64, device=dev) \
+            if self.multi else None
         # ---- reused device buffers
         # ONE lookup buffer: every run rebuilds it in stream order, after the previous run's scan.  (Two
         # alternating buffers would keep both sets of evict_last lines next to the group tables, and a step
@@ -1746,6 +1758,10 @@ class PreparedStar:
         # the 4 flag words share it: one broadcast carries them all.
         self.slot_bits = _star_slot_bits(self.nslots - 1)
         slots_off, self.flags_off, words = _star_bitmap_words(q.prange, q.dn, self.slot_bits)
+        # 21-bit slots are stored as int32 into a staging array of this many entries and packed from it
+        # (b2_star_build_pack).  run() takes it from the caching allocator for the build only: held by the plan,
+        # 20 MB for C4 would stay resident between runs for nothing.
+        self.stage_n = min(q.dn, q.prange) if self.slot_bits == 21 and not per_part else 0
         self.lookup = torch.empty(words, dtype=torch.int32, device=dev)
         self.lk = lk = L.StarLookup()
         lk.dense, lk.dir, lk.kmin, lk.range, lk.slot_bits = 2, self.lookup.data_ptr(), q.pmin, q.prange, self.slot_bits
@@ -1892,8 +1908,10 @@ class PreparedStar:
         # cost.)
         if q.owner:
             with _Phase("build"):
+                stage = torch.empty(self.stage_n, dtype=torch.int32, device=self.dev) if self.stage_n else None
                 _star_bitmap_build(buf, self.dim_launch, q.pmin, q.prange, q.gmin, self.nslots - 1, q.dn,
-                                   self.slot_bits, sp)
+                                   self.slot_bits, sp, stage)
+                del stage          # back to the allocator; reused only in stream order, after the pack
         if q.bcast:
             # the build side crosses NVLink as the finished lookup (directory + slots), not as its columns
             with _Phase("bcast"):
@@ -1905,12 +1923,26 @@ class PreparedStar:
             if self.dirty[ti]:
                 t.reset()
             self.dirty[ti] = True
-            for scan, bases, fk_slot, aggs_arr, naggs, n in self.fact_launch:
-                stats["launches"] += 1
-                ev = _kernel_event_begin("b2_star_agg_kernel", n)
-                L.star_agg_narrow(C.byref(scan), bases, fk_slot, C.byref(self.lk), aggs_arr, naggs, C.byref(t.state),
-                                  sp)
+            if self.multi:
+                fl = self.fact_launch
+                scans = (L.Scan * len(fl))(*[launch[0] for launch in fl])
+                bases = (C.c_void_p * len(fl))(*[None if launch[1] is None else C.addressof(launch[1])
+                                                  for launch in fl])
+                _, _, fk_slot, aggs_arr, naggs, _ = fl[0]
+                tk = C.c_void_p(self.tickets.data_ptr())
+                L.memset(tk, 0, 8 * self.tickets.numel(), sp)
+                stats["launches"] += self.tickets.numel()
+                ev = _kernel_event_begin("b2_star_agg_kernel", self.fact_rows)
+                L.star_agg_multi(scans, bases, len(fl), fk_slot, C.byref(self.lk), aggs_arr, naggs, C.byref(t.state),
+                                 tk, sp)
                 _kernel_event_end(ev)
+            else:
+                for scan, bases, fk_slot, aggs_arr, naggs, n in self.fact_launch:
+                    stats["launches"] += 1
+                    ev = _kernel_event_begin("b2_star_agg_kernel", n)
+                    L.star_agg_narrow(C.byref(scan), bases, fk_slot, C.byref(self.lk), aggs_arr, naggs,
+                                      C.byref(t.state), sp)
+                    _kernel_event_end(ev)
         if self.peer is not None:
             m, view = self.peer[ti]
             self.epoch += 1
@@ -1970,24 +2002,29 @@ def _star_bitmap_words(prange, dn, slot_bits):
     return slots, flags, flags + 4
 
 
-def _star_bitmap_build(buf, launches, pmin, prange, gmin, null_slot, dn, slot_bits, sp):
+def _star_bitmap_build(buf, launches, pmin, prange, gmin, null_slot, dn, slot_bits, sp, stage=None):
     """The ranked-bitmap lookup from (scan, image bases, pk slot, grp slot) of every dim partition, in stream order:
-    zero the directory (with packed slots, the slot words too: FILL ORs into them) and flags, mark every
-    partition, rank, fill every partition."""
+    zero the directory (with packed slots filled in place, the slot words too: FILL ORs into them) and flags,
+    mark every partition, rank, fill every partition.  `stage` (21-bit slots only):
+    the fill stores plain int32 entries into it, and b2_star_build_pack packs them into every slot word."""
     slots_off, flags_off, _ = _star_bitmap_words(prange, dn, slot_bits)
     base = buf.data_ptr()
     dirp, slots, flags = C.c_void_p(base), C.c_void_p(base + 4 * slots_off), C.c_void_p(base + 4 * flags_off)
-    L.memset(dirp, 0, 4 * (flags_off if slot_bits < 32 else slots_off), sp)
+    L.memset(dirp, 0, 4 * (flags_off if slot_bits < 32 and stage is None else slots_off), sp)
     L.memset(flags, 0, 16, sp)
     for scan, bases, pk_slot, _ in launches:
         stats["launches"] += 1
         L.star_build_mark_narrow(C.byref(scan), bases, pk_slot, pmin, prange, dirp, flags, sp)
     stats["launches"] += 1
     L.star_build_rank(dirp, prange, sp)
+    fill_to, fill_bits = (slots, slot_bits) if stage is None else (C.c_void_p(stage.data_ptr()), 32)
     for scan, bases, pk_slot, g_slot in launches:
         stats["launches"] += 1
-        L.star_build_fill_narrow(C.byref(scan), bases, pk_slot, g_slot, pmin, prange, gmin, null_slot, dirp, slots,
-                                 slot_bits, sp)
+        L.star_build_fill_narrow(C.byref(scan), bases, pk_slot, g_slot, pmin, prange, gmin, null_slot, dirp, fill_to,
+                                 fill_bits, sp)
+    if stage is not None:
+        stats["launches"] += 1
+        L.star_build_pack(dirp, prange, C.c_void_p(stage.data_ptr()), stage.numel(), slots, slot_bits, sp)
 
 
 def _star_dense_fast(src, fact, dim, fk_e, pk_e, gexprs, aggs, fact_pred, dim_pred, sharded, dev) -> Optional[Part]:

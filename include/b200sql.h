@@ -633,6 +633,12 @@ int32_t b2_star_build_mark_narrow(const b2_scan_t* scan, const int64_t* bases, i
 int32_t b2_star_build_fill_narrow(const b2_scan_t* scan, const int64_t* bases, int32_t pk_col, int32_t grp_col,
                                   int64_t pk_min, int64_t pk_range, int64_t grp_min, int32_t null_slot,
                                   const uint64_t* dir, uint64_t* slots, int32_t slot_bits, void* stream);
+/* The 21-bit slots without a CAS per entry: b2_star_build_fill_narrow with slot_bits = 32 into `staged`
+ * (int32[capacity], capacity = the entries of the slots array), where a duplicate pk's last store wins, then
+ * this pack of `staged` into the 3-per-word slots array (ceil(capacity / 3) words, all of them written, so
+ * they need no zeroing; entries past the last set bit of `dir` are 0).  Only slot_bits == 21. */
+int32_t b2_star_build_pack(const uint64_t* dir, int64_t pk_range, const int32_t* staged, int64_t capacity,
+                           uint64_t* slots, int32_t slot_bits, void* stream);
 /* Hash variant: table_keys = int64[cap] pre-filled with B2_EMPTY_KEY, table_slots = int32[cap].
  * d_flags[0] = 1 on duplicate pk, d_flags[1] = 1 on overflow. */
 int32_t b2_star_build_hash(const b2_col_t* pk, const int32_t* sel, int64_t n_sel,
@@ -660,6 +666,15 @@ int32_t b2_star_agg(const b2_scan_t* scan, int32_t fk_col, const b2_starlookup_t
 /* b2_star_agg over a scan that may hold B2_U32 images, bases[] as for b2_star_build_mark_narrow */
 int32_t b2_star_agg_narrow(const b2_scan_t* scan, const int64_t* bases, int32_t fk_col, const b2_starlookup_t* lk,
                            const b2_agg_t* aggs, int32_t naggs, const b2_aggstate_t* st, void* stream);
+/* b2_star_agg_narrow over nparts partitions of one table (scans[i], bases[i]; bases or bases[i] NULL: no
+ * images), with one launch per B2_STAR_MAX_PARTS partitions instead of one per partition: tiles of every
+ * partition in the launch share one persistent grid, and the tail is handed out by a ticket.  fk_col and
+ * the aggregates index every scan alike.  d_tickets: ceil(nparts / B2_STAR_MAX_PARTS) uint64 words, zero
+ * at the call in stream order.  st->out_slot, indexed by the row within a partition, only with nparts <= 1. */
+#define B2_STAR_MAX_PARTS 16
+int32_t b2_star_agg_multi(const b2_scan_t* scans, const int64_t* const* bases, int32_t nparts, int32_t fk_col,
+                          const b2_starlookup_t* lk, const b2_agg_t* aggs, int32_t naggs, const b2_aggstate_t* st,
+                          uint64_t* d_tickets, void* stream);
 
 #ifdef __cplusplus
 }

@@ -1,14 +1,17 @@
 #!/usr/bin/env python
 """Where a C4 step goes on one GPU: the bench.py headline query (same generator and seeds, 1e9 fact rows
 in 8 partitions, 10M dim rows, 1M groups) timed with CUDA events per phase of PreparedStar.run (build /
-scan / ...) and per launch of the ranked-bitmap build (the memsets, every mark, the rank, every fill),
-next to the step time and the b2_star_agg_kernel time.  One JSON line per phase and per launch, in ms
+scan / ...) and per launch of the ranked-bitmap build (the memsets, every mark, the rank, every fill, and the pack of the
+staged 21-bit slots), next to the step time and the b2_star_agg_kernel time: one launch per step over all 8
+fact partitions (b2_star_agg_multi), or one per partition with B200SQL_STAR_PER_PART=1, whose fill updates
+the packed slots in place by CAS and has no pack.  One JSON line per phase and per launch, in ms
 per step and per call, each carrying the card's name and power limit; then one "bytes" line: the bytes per
 fact and per dim row that the prepared plan's scans physically read (int64 columns streamed as their 32-bit
 images, DeviceColumn.star_image, unless B200SQL_NO_NARROW=1) against the logical 24 B per fact row that
 bench.py's roofline divides by, and the probe's physical bandwidth from the b2_star_agg_kernel time.
 
     python scripts/star_step_breakdown.py --steps 10 --warmup 3
+    B200SQL_STAR_PER_PART=1 python scripts/star_step_breakdown.py --steps 10 --warmup 3
     B200SQL_NO_NARROW=1 python scripts/star_step_breakdown.py --steps 10 --warmup 3
 
 B200SQL_LIB selects another build of libb200sql.so (the C-ABI is the same), so two builds can be
@@ -47,7 +50,8 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--label", default=os.environ.get("B200SQL_LIB", "in-tree") +
-                    (" int64" if os.environ.get("B200SQL_NO_NARROW") == "1" else " images"))
+                    (" int64" if os.environ.get("B200SQL_NO_NARROW") == "1" else " images") +
+                    (" per-partition" if os.environ.get("B200SQL_STAR_PER_PART") == "1" else ""))
     args = ap.parse_args()
     if args.steps < 1:
         ap.error("--steps must be >= 1")
@@ -91,7 +95,7 @@ def main():
         return call
 
     for attr, name in (("memset", "memset"), ("star_build_mark_narrow", "mark"), ("star_build_rank", "rank"),
-                       ("star_build_fill_narrow", "fill")):
+                       ("star_build_fill_narrow", "fill"), ("star_build_pack", "pack")):
         setattr(L, attr, timed(name, getattr(L, attr)))
     build = executor._star_bitmap_build
 
