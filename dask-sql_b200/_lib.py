@@ -94,6 +94,14 @@ PEER_SUM_F64, PEER_SUM_I64, PEER_MIN_I64, PEER_MAX_I64, PEER_AND_I64, PEER_OR_I6
 PEER_PRESENT_ROWS, PEER_PRESENT_INDICATOR, PEER_PRESENT_BITMAP = 1, 2, 3
 
 
+SELECT_MAX_TARGETS, SELECT_MAX_BITS = 8, 11
+
+
+class Select(C.Structure):
+    _fields_ = [("prefix", C.c_uint64 * SELECT_MAX_TARGETS), ("nsel", C.c_int32), ("shift", C.c_int32),
+                ("bits", C.c_int32), ("pad_", C.c_int32)]
+
+
 class PeerMerge(C.Structure):
     _fields_ = [("world", C.c_int32), ("rank", C.c_int32), ("narrays", C.c_int32), ("presence_kind", C.c_int32),
                 ("presence_array", C.c_int32), ("ops", C.c_int32 * PEER_MAX_ARRAYS),
@@ -106,6 +114,7 @@ class PeerMerge(C.Structure):
 assert C.sizeof(Col) == 24 and C.sizeof(Term) == 32 and C.sizeof(Scan) == 656
 assert C.sizeof(AggState) == 152 and C.sizeof(Instr) == 24 and C.sizeof(Prog) == 1544
 assert C.sizeof(JoinTable) == 152 and C.sizeof(StarLookup) == 64 and C.sizeof(PeerMerge) == 544
+assert C.sizeof(Select) == 80
 
 
 def agg_identity(op):
@@ -196,6 +205,7 @@ _SIGS = {
     "b2_bitwise_combine": [_P, _P, C.c_int64, C.c_int32, _P],
     "b2_peer_merge": [C.POINTER(PeerMerge), _P],
     "b2_sort_by": [C.POINTER(Col), C.c_int64, C.c_int32, C.c_int32, _P, _P, _P],
+    "b2_select_hist": [C.POINTER(Col), C.c_int64, C.POINTER(Select), _P, _P, _P, _P],
     "b2_dense_slots": [C.POINTER(Col), C.c_int64, C.c_int64, C.c_int32, _P, _P],
     "b2_narrow_image": [C.POINTER(Col), C.c_int64, C.c_int64, _P, _P],
     "b2_star_build_dense": [C.POINTER(Col), _P, C.c_int64, _P, C.c_int64, C.c_int64, _P, _P, _P],
@@ -299,6 +309,7 @@ sort_by = _wrap("b2_sort_by")
 _lib.b2_sort_ws_bytes.restype = C.c_int64
 _lib.b2_sort_ws_bytes.argtypes = [C.c_int64]
 sort_ws_bytes = _lib.b2_sort_ws_bytes
+select_hist = _wrap("b2_select_hist")
 dense_slots = _wrap("b2_dense_slots")
 narrow_image = _wrap("b2_narrow_image")
 star_build_dense = _wrap("b2_star_build_dense")

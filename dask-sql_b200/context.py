@@ -51,7 +51,7 @@ class Context:
         # replace=False: whoever registered a plugin for a node type before us -- or registers one
         # later with replace=True -- wins (context.py:118-158); that is the drop-in seam
         for plugin in (*logical.ALL_PLUGINS, custom.CreateMemoryTablePlugin, custom.CreateTablePlugin,
-                       custom.DropTablePlugin):
+                       custom.DropTablePlugin, custom.AnalyzeTablePlugin):
             RelConverter.add_plugin_class(plugin, replace=False)
         for plugin in core.ALL_PLUGINS:
             RexConverter.add_plugin_class(plugin, replace=False)
@@ -242,8 +242,8 @@ class Context:
 
     def _compute_table_from_rel(self, rel, return_futures: bool = True):
         dc = RelConverter.convert(rel, context=self)
-        if rel.get_current_node_type() == "Explain":
-            return dc
+        if rel.get_current_node_type() in ("Explain", "AnalyzeTable"):
+            return dc      # the plan text / the statistics frame, already on the host
         if dc is None:
             return
         # keep alias projects; FQ name only where the simple name is ambiguous (context.py:882-906)

@@ -37,6 +37,7 @@ int b2_sm_count() {
 #include "join.cuh"
 #include "joinagg.cuh"
 #include "sort.cuh"
+#include "select.cuh"
 #include "partition.cuh"
 #include "peer.cuh"
 #include "strings.cuh"

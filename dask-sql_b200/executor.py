@@ -573,6 +573,139 @@ def run_sort(src: SortSource, needed: Set[str]) -> Part:
     return out
 
 
+_SIGN = 1 << 63
+_U64 = (1 << 64) - 1
+
+
+def select_image(value, dtype) -> int:
+    """The unsigned order-preserving image b2_select_hist histograms, of a non-NULL int64 / float64 value."""
+    key = int(value) if dtype == I64 else int(L.f64_to_ordered(float(value)))
+    return (key & _U64) ^ _SIGN
+
+
+def _signed(x: int) -> int:
+    return x - (1 << 64) if x >= _SIGN else x
+
+
+def select_value(image: int, dtype):
+    """select_image inverted: the int64 / float64 value of an image."""
+    key = _signed(image ^ _SIGN)
+    return key if dtype == I64 else L.ordered_to_f64(key)
+
+
+def order_statistics(cols: Sequence[DeviceColumn], dtype: int, ranks: Sequence[int], umin: int, umax: int, count: int,
+                     sharded: bool = False) -> Dict[int, int]:
+    """k -> image of the k-th smallest (0-based) non-NULL, non-NaN value, for every k in ranks, of the column
+    whose partitions are `cols` (all of `dtype`, I64 or F64).  umin / umax: images of its min and max, count: its
+    non-NULL rows (over every rank when sharded).
+
+    MSD radix select with b2_select_hist: starting at the highest bit where umin and umax differ, each pass
+    takes up to SELECT_MAX_BITS bits over every partition, then each target's histogram is walked to the digit
+    that holds its rank.  Targets that still share a prefix share a histogram.  Once the rows sharing some
+    target's prefix are at most count / 8, the next pass that is not the last also copies them to a dense
+    buffer, and the passes after it read that buffer instead of the column.  sharded: each pass's histograms
+    are summed over the ranks (parallel.allreduce_) before the walk, so every rank picks the same digits."""
+    targets = sorted({int(k) for k in ranks})
+    if not targets:
+        return {}
+    if not 0 <= targets[0] <= targets[-1] < count:
+        raise ValueError(f"ranks {targets} outside a column of {count} values")
+    diff = umin ^ umax
+    if diff == 0:
+        return {k: umin for k in targets}
+    dev = _dev()
+    level = diff.bit_length()              # shift + bits of the first pass
+    prefix = {k: umin >> level if level < 64 else 0 for k in targets}
+    rank = {k: k for k in targets}
+    src = [c for c in cols if c.n]
+    matched = local_matched = None         # rows in the buckets the previous pass chose (all ranks / this one)
+    compacted = False
+    while level > 0:
+        bits = min(L.SELECT_MAX_BITS, level)
+        shift = level - bits
+        groups = sorted(set(prefix.values()))
+        sel = L.Select()
+        sel.nsel, sel.shift, sel.bits = len(groups), shift, bits
+        for g, p in enumerate(groups):
+            sel.prefix[g] = p
+        hist = torch.zeros(len(groups) << bits, dtype=torch.int64, device=dev)
+        out = n_out = None
+        if not compacted and shift > 0 and matched is not None and 8 * matched <= count:
+            out = torch.empty(max(local_matched, 1), dtype=torch.int64, device=dev)
+            n_out = torch.zeros(1, dtype=torch.int64, device=dev)
+        rec = _kernel_event_begin("b2_select_hist" if out is None else "b2_select_hist_compact",
+                                  sum(c.n for c in src))
+        for c in src:
+            cs = c.as_struct()
+            stats["launches"] += 1
+            L.select_hist(C.byref(cs), c.n, C.byref(sel), D.ptr(hist), D.ptr(out), D.ptr(n_out), D.stream_ptr())
+        _kernel_event_end(rec)
+        stats["select_passes"] = stats.get("select_passes", 0) + 1
+        local = hist.cpu().numpy().reshape(len(groups), 1 << bits)
+        if sharded:
+            P.allreduce_(hist)
+        h = hist.cpu().numpy().reshape(len(groups), 1 << bits) if sharded else local
+        if out is not None:
+            src = [DeviceColumn(out[:local_matched], None, dtype)] if local_matched else []
+            compacted = True
+            stats["select_compactions"] = stats.get("select_compactions", 0) + 1
+        chosen = set()
+        for k in targets:
+            g = groups.index(prefix[k])
+            cum = np.cumsum(h[g])
+            d = int(np.searchsorted(cum, rank[k], side="right"))
+            if d == len(cum):
+                raise RuntimeError(f"order statistic {k}: {int(cum[-1])} rows share its prefix; the column "
+                                   "statistics do not describe the column")
+            rank[k] -= int(cum[d] - h[g][d])
+            chosen.add((g, d))
+            prefix[k] = (prefix[k] << bits) | d
+        matched = sum(int(h[g][d]) for g, d in chosen)
+        local_matched = sum(int(local[g][d]) for g, d in chosen)
+        level = shift
+    return prefix
+
+
+def column_quantiles(table: DeviceTable, name: str, qs: Sequence[float] = (0.25, 0.5, 0.75)):
+    """count, min, max and the exact linear-interpolation quantiles of one int64 / float64 column of a table,
+    NULL and NaN excluded: (count, vmin, vmax, [(x_lo, x_hi, gamma) per q]), values as python int / float,
+    min / max / x_* None when count == 0.  Quantile q sits at virtual index q * (count - 1) as in pandas:
+    x_lo is the order statistic at its floor, x_hi the next one (clamped), gamma the fraction; the caller
+    interpolates them.  Sharded and 'root' tables: every rank returns the same answer."""
+    dtype = dict((n, d) for n, d, _ in table.schema())[name]
+    if dtype not in (I64, F64):
+        raise TypeError(f"column {name!r}: order statistics need an int64 or float64 column")
+    st = table.column_stats(name)
+    count = table.nrows - st.nulls
+    umin = _U64 if st.vmin is None else select_image(st.vmin, dtype)
+    umax = 0 if st.vmin is None else select_image(st.vmax, dtype)
+    if dtype == F64 and st.vmin is not None:
+        # -0.0 and +0.0 have distinct images: start the walk below either zero that min / max may stand for
+        umin = min(umin, select_image(-0.0, dtype)) if st.vmin == 0.0 else umin
+        umax = max(umax, select_image(0.0, dtype)) if st.vmax == 0.0 else umax
+    sharded = P.world()[1] > 1 and table.distribution in ("sharded", "root")
+    if sharded:
+        # images cross the collective as signed keys (image ^ 2^63), whose signed order is the image order
+        cnt, lo, hi = (torch.tensor([v], dtype=torch.int64, device=_dev())
+                       for v in (count, _signed(umin ^ _SIGN), _signed(umax ^ _SIGN)))
+        P.allreduce_(cnt)
+        P.allreduce_(lo, "min")
+        P.allreduce_(hi, "max")
+        count = int(cnt.item())
+        umin, umax = (int(lo.item()) & _U64) ^ _SIGN, (int(hi.item()) & _U64) ^ _SIGN
+    if count == 0:
+        return 0, None, None, [(None, None, float("nan")) for _ in qs]
+    ranks = []
+    for q in qs:
+        pos = q * (count - 1)
+        lo = int(np.floor(pos))
+        ranks.append((lo, min(lo + 1, count - 1), pos - lo))
+    cols = [p[name] for p in materialize(TableSource(table), {name}) if p.n]
+    img = order_statistics(cols, dtype, [k for lo, hi, _ in ranks for k in (lo, hi)], umin, umax, count, sharded)
+    return (count, select_value(umin, dtype), select_value(umax, dtype),
+            [(select_value(img[lo], dtype), select_value(img[hi], dtype), g) for lo, hi, g in ranks])
+
+
 def run_limit(src: LimitSource, needed: Set[str]) -> Part:
     dev = _dev()
     names = [n for n in src.child.columns if n in needed]

@@ -1,7 +1,8 @@
-"""Statements around the path: CREATE TABLE ... WITH / AS, CREATE VIEW ... AS, DROP TABLE
+"""Statements around the path: CREATE TABLE ... WITH / AS, CREATE VIEW ... AS, DROP TABLE, ANALYZE TABLE
 (dask_sql/physical/rel/custom/)."""
+from .analyze_table import AnalyzeTablePlugin
 from .create_memory_table import CreateMemoryTablePlugin
 from .create_table import CreateTablePlugin
 from .drop_table import DropTablePlugin
 
-__all__ = [CreateMemoryTablePlugin, CreateTablePlugin, DropTablePlugin]
+__all__ = [AnalyzeTablePlugin, CreateMemoryTablePlugin, CreateTablePlugin, DropTablePlugin]

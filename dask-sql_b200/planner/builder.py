@@ -57,7 +57,30 @@ class Binder:
             return P.CreateTable(node.name, node.kwargs, node.or_replace, node.if_not_exists)
         if node.kind == "drop_table":
             return P.DropTable(node.name, node.if_exists)
+        if node.kind == "analyze_table":
+            return self.bind_analyze(node)
         return self.bind_query(node, {})
+
+    def bind_analyze(self, node: Node) -> P.LogicalPlan:
+        parts = node.name.split(".")
+        schema_name, table_name = (parts[-2], parts[-1]) if len(parts) >= 2 else (None, parts[0])
+        found = self.catalog(schema_name, table_name)
+        if found is None:
+            self.err(f"Error during planning: table '{node.name}' not found")
+        schema_name, cols = found
+        names = [c for c, _ in cols]
+        columns = []
+        for c in node.columns:
+            hits = [n for n in names if n == c]
+            if not hits and not self.case_sensitive:
+                hits = [n for n in names if n.lower() == c.lower()]
+            if len(hits) != 1:
+                self.err(f"Column '{c}' not found in table '{node.name}'" if not hits else
+                         f"Column '{c}' is ambiguous in table '{node.name}'")
+            if hits[0] in columns:
+                self.err(f"Column '{c}' is listed more than once in ANALYZE TABLE")
+            columns.append(hits[0])
+        return P.AnalyzeTable(schema_name, table_name.lower(), columns, columns or names)
 
     def bind_query(self, q: Node, ctes: Dict[str, P.LogicalPlan]) -> P.LogicalPlan:
         ctes = dict(ctes)

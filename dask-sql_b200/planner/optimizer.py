@@ -213,7 +213,7 @@ def optimize(plan: P.LogicalPlan) -> P.LogicalPlan:
     if isinstance(plan, (P.Explain, P.CreateMemoryTable)):
         plan.inputs = [optimize(plan.inputs[0])]
         return plan
-    if isinstance(plan, (P.CreateTable, P.DropTable)):
+    if isinstance(plan, (P.CreateTable, P.DropTable, P.AnalyzeTable)):
         return plan
     plan = push_filters(plan, [])
     plan = prune_columns(plan)

@@ -790,6 +790,33 @@ class DropTable(LogicalPlan):
         return f"DropTable: {self.name}"
 
 
+class AnalyzeTable(LogicalPlan):
+    """ANALYZE TABLE name COMPUTE STATISTICS FOR ALL COLUMNS | COLUMNS c1, ... (src/sql/logical/analyze_table.rs;
+    custom/analyze_table.py).  The table and the listed columns are resolved at planning; getColumns() is
+    empty for ALL COLUMNS."""
+    node_type = "AnalyzeTable"
+
+    def __init__(self, schema_name, table_name, columns, fields):
+        super().__init__([])
+        self.schema_name, self.table_name, self.columns = schema_name, table_name, list(columns)
+        self.schema = [RelDataTypeField(None, f, "VARCHAR", i) for i, f in enumerate(fields)]
+
+    def analyze_table(self):
+        return self
+
+    def getSchemaName(self):
+        return self.schema_name
+
+    def getTableName(self):
+        return self.table_name
+
+    def getColumns(self):
+        return list(self.columns)
+
+    def describe(self):
+        return f"AnalyzeTable: {self.schema_name}.{self.table_name} {self.columns or 'ALL COLUMNS'}"
+
+
 def walk(plan: LogicalPlan):
     yield plan
     for i in plan.inputs:

@@ -20,7 +20,9 @@ Statements around the path (custom statements of the reference's parser, src/par
   CREATE [OR REPLACE] TABLE|VIEW [IF NOT EXISTS] [schema.]name AS [(] query [)]
   CREATE [OR REPLACE] TABLE [IF NOT EXISTS] [schema.]name WITH (key = literal [, ...])
   DROP TABLE [IF EXISTS] [schema.]name
-CREATE / DROP / TABLE / VIEW / IF / EXISTS / REPLACE are contextual words, not reserved.
+  ANALYZE TABLE [schema.]name COMPUTE STATISTICS FOR ALL COLUMNS | COLUMNS c1 [, c2 ...]
+CREATE / DROP / TABLE / VIEW / IF / EXISTS / REPLACE / ANALYZE / COMPUTE / STATISTICS / FOR / COLUMNS are
+contextual words, not reserved.
 """
 import re
 from typing import List, Optional
@@ -161,6 +163,22 @@ class Parser:
 
     # -- statements
     def parse_ddl(self) -> Optional[Node]:
+        if self.at_word("ANALYZE") and self.toks[self.i + 1].kind == "id":
+            self.i += 1
+            self.expect_word("TABLE")
+            name = self.qualified_name()
+            self.expect_word("COMPUTE")
+            self.expect_word("STATISTICS")
+            self.expect_word("FOR")
+            columns = []
+            if self.eat_kw("ALL"):
+                self.expect_word("COLUMNS")
+            else:
+                self.expect_word("COLUMNS")
+                columns.append(self.ident())
+                while self.eat_op(","):
+                    columns.append(self.ident())
+            return Node("analyze_table", name=name, columns=columns)
         if self.at_word("DROP") and self.toks[self.i + 1].kind == "id":
             self.i += 1
             self.expect_word("TABLE")

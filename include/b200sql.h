@@ -583,6 +583,30 @@ int32_t b2_iota(int32_t* out, int64_t n, void* stream);
 int32_t b2_sort_by(const b2_col_t* col, int64_t n, int32_t descending, int32_t nulls_first, int32_t* idx,
                    void* ws, void* stream);
 
+/* ---- exact order statistics (ANALYZE TABLE ... COMPUTE STATISTICS quantiles) -------------------- */
+/* One pass of a multi-target MSD radix select over one B2_I64 or B2_F64 column (any other dtype is
+ * B2_ERR_ARG).  Rows whose validity bit is clear, and float NaN, are skipped.  Every other row has the
+ * unsigned order-preserving image u (int64: sign bit flipped; float64: b2_ordered_from_bits, sign bit
+ * flipped, so -0.0 sorts just below +0.0).  For each target k < nsel whose prefix matches,
+ * u >> (shift + bits) == prefix[k] (every row when shift + bits == 64, where prefix[k] must be 0):
+ *   hist[k * 2^bits + ((u >> shift) & (2^bits - 1))] += 1      (hist: uint64, accumulated, zeroed by the caller)
+ * out != NULL makes the pass compact: the raw 64-bit value of every row that matches some target's
+ * prefix is written to out[atomic (*out_count)++], in no particular order, so that later passes read
+ * that dense buffer as a column of the same dtype without a bitmap.  Size it from the previous pass's
+ * histogram: the sum of the buckets the targets chose.
+ * Replaces the quantiles of describe() in physical/rel/custom/analyze_table.py. */
+#define B2_SELECT_MAX_TARGETS 8
+#define B2_SELECT_MAX_BITS   11
+typedef struct b2_select {
+  uint64_t prefix[B2_SELECT_MAX_TARGETS];
+  int32_t  nsel;    /* 1 .. B2_SELECT_MAX_TARGETS */
+  int32_t  shift;   /* >= 0, shift + bits <= 64 */
+  int32_t  bits;    /* 1 .. B2_SELECT_MAX_BITS */
+  int32_t  pad_;
+} b2_select_t;
+int32_t b2_select_hist(const b2_col_t* col, int64_t n, const b2_select_t* sel, uint64_t* hist, int64_t* out,
+                       uint64_t* out_count, void* stream);
+
 /* ---- fused filter -> join -> group-by (star pipeline) ----------------------------- */
 /* out_slot[i] = key[i]-kmin (NULL key -> null_slot) as int32: turns a dense group-key column of
  * the build side into group-table slot numbers. */

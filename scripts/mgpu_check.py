@@ -159,6 +159,24 @@ def main():
     dist.all_reduce(t)
     assert int(t[0]) == n_unmatched_exp, (int(t[0]), n_unmatched_exp)
     assert int(t[1]) == nf, (int(t[1]), nf)         # every probe row appears once (NULL-fk rows unmatched)
+    # 6. ANALYZE on the sharded table: the select's histograms are summed over the ranks, so every rank returns
+    # the frame one GPU computes from the whole table
+    sql = "ANALYZE TABLE fact COMPUTE STATISTICS FOR ALL COLUMNS"
+    got = c.sql(sql)
+    c5 = Context()
+    c5.create_table("fact", fact, persist=True, npartitions=3)
+    one = c5.sql(sql)
+    frames = [None] * world
+    dist.all_gather_object(frames, got)
+    for f in frames:
+        assert list(f.columns) == list(one.columns) and list(f.index) == list(one.index)
+        for col in one.columns:
+            for row in one.index:
+                a, b = f.at[row, col], one.at[row, col]
+                if row in ("mean", "std"):
+                    assert (pd.isna(a) and pd.isna(b)) or abs(a - b) <= 1e-9 * max(1.0, abs(b)), (col, row, a, b)
+                else:
+                    assert (pd.isna(a) and pd.isna(b)) or a == b, (col, row, a, b)
     dist.barrier()
     if rank == 0:
         print(f"mgpu_check OK on {world} GPUs")
