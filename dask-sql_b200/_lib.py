@@ -27,6 +27,7 @@ OP_EQ_I, OP_EQ_F = 30, 40
 OP_AND, OP_OR, OP_NOT, OP_ISNULL_I, OP_ISNULL_F, OP_CASE, OP_FILLNA, OP_ORD2F = 50, 51, 52, 53, 54, 55, 56, 57
 OP_DATEPART, OP_ADDMONTHS, OP_MAP = 60, 61, 62
 OP_MATH_F, OP_MATH2_F, OP_POW_I = 63, 64, 65
+OP_RAND_F, OP_RAND_I = 66, 67
 # B2_OP_MATH_F / B2_OP_MATH2_F functions (b200sql.h B2_FN_*)
 (FN_CEIL, FN_FLOOR, FN_TRUNC, FN_ROUND, FN_SIGN, FN_DEGREES, FN_RADIANS, FN_EXP, FN_LN, FN_LOG10, FN_CBRT, FN_SIN,
  FN_COS, FN_TAN, FN_COT, FN_ASIN, FN_ACOS, FN_ATAN, FN_ATAN2, FN_POW, FN_MOD) = range(21)
@@ -158,6 +159,7 @@ _SIGS = {
     "b2_memset": [_P, C.c_int32, C.c_int64, _P],
     "b2_col_stats": [C.POINTER(Col), C.c_int64, _P, _P, _P],
     "b2_expr_eval": [C.POINTER(Prog), C.POINTER(Col), C.c_int32, C.c_int64, _P, _P, _P],
+    "b2_expr_eval_rows": [C.POINTER(Prog), C.POINTER(Col), C.c_int32, C.c_int64, C.c_int64, _P, _P, _P],
     "b2_scan_agg": [C.POINTER(Scan), C.POINTER(Agg), C.c_int32, _P, _P, C.c_int32, _P, _P],
     "b2_select_count": [C.POINTER(Scan), _P, _P],
     "b2_select_write": [C.POINTER(Scan), _P, _P, C.c_int32, C.POINTER(C.c_int32), C.POINTER(_P),
@@ -226,6 +228,7 @@ _SIGS = {
     "b2_star_agg_multi": [C.POINTER(Scan), _P, C.c_int32, C.c_int32, C.POINTER(StarLookup), C.POINTER(Agg), C.c_int32,
                           C.POINTER(AggState), _P, _P],
     "b2_star_build_pack": [_P, C.c_int64, _P, C.c_int64, _P, C.c_int32, _P],
+    "b2_sample_mask": [C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int64, _P, _P],
     "b2_str_like": [_P, _P, C.c_int64, _P, C.c_int64, C.c_uint32, C.c_int32, _P, _P],
     "b2_str_lower_bound": [_P, _P, C.c_int64, _P, _P, C.c_int64, C.c_int32, _P, _P, _P],
 }
@@ -277,6 +280,7 @@ sync = _wrap("b2_sync")
 memset = _wrap("b2_memset")
 col_stats = _wrap("b2_col_stats")
 expr_eval = _wrap("b2_expr_eval")
+expr_eval_rows = _wrap("b2_expr_eval_rows")
 scan_agg = _wrap("b2_scan_agg")
 select_count = _wrap("b2_select_count")
 select_write = _wrap("b2_select_write")
@@ -324,6 +328,7 @@ star_build_fill_narrow = _wrap("b2_star_build_fill_narrow")
 star_agg_narrow = _wrap("b2_star_agg_narrow")
 star_agg_multi = _wrap("b2_star_agg_multi")
 star_build_pack = _wrap("b2_star_build_pack")
+sample_mask = _wrap("b2_sample_mask")
 str_like = _wrap("b2_str_like")
 str_lower_bound = _wrap("b2_str_lower_bound")
 num_tiles = _lib.b2_num_tiles

@@ -131,6 +131,7 @@ class Context:
             table.name = table_name
             df = LazyFrame(TableSource(table))
         dc = DataContainer(df, ColumnContainer(df.columns))
+        dc.view = isinstance(input_table, LazyFrame) and not persist    # no row numbers to sample by
         if not statistics:
             statistics = Statistics(float("nan"))
         dc.statistics = statistics
@@ -185,7 +186,7 @@ class Context:
                 if df is None:
                     rel, _ = self._get_ral(sql)
                     df = self._compute_table_from_rel(rel, True)
-                    if isinstance(df, LazyFrame):
+                    if isinstance(df, LazyFrame) and not getattr(rel, "volatile", False):
                         if len(self._plan_cache) > 256:
                             self._plan_cache.clear()
                         self._plan_cache[key] = df

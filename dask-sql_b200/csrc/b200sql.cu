@@ -31,6 +31,7 @@ int b2_sm_count() {
   return g_sm_count_cache[dev];
 }
 
+#include "rand.cuh"
 #include "expr.cuh"
 #include "filter.cuh"
 #include "groupby.cuh"

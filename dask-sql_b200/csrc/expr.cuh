@@ -4,6 +4,7 @@
 // space), so the interpreter loop never diverges; the value stack lives in local memory.
 #pragma once
 #include "common.cuh"
+#include "rand.cuh"
 
 #define B2_STACK 16
 
@@ -142,7 +143,7 @@ __device__ __noinline__ int64_t b2_pow_i(int64_t x, int64_t y) {   // y >= 0; wr
 
 __global__ void __launch_bounds__(B2_BLOCK)
 b2_expr_kernel(const __grid_constant__ b2_prog_t prog, const __grid_constant__ b2_cols_arg cols,
-               int64_t n, void* __restrict__ out_data, uint32_t* __restrict__ out_valid) {
+               int64_t n, int64_t row_base, void* __restrict__ out_data, uint32_t* __restrict__ out_valid) {
   const int64_t n32 = (n + 31) & ~(int64_t)31;
   for (int64_t row = (int64_t)blockIdx.x * B2_BLOCK + threadIdx.x; row < n32;
        row += (int64_t)gridDim.x * B2_BLOCK) {
@@ -215,6 +216,15 @@ b2_expr_kernel(const __grid_constant__ b2_prog_t prog, const __grid_constant__ b
           sn[sp - 1] = !hit;
         } else if (op == B2_OP_MATH_F) {
           sv[sp - 1] = b2_math_f(sv[sp - 1], ins.a, ins.imm_f, ins.imm_i);
+        } else if (op == B2_OP_RAND_F) {
+          const uint64_t u = b2_rand_u64(row_base + row, ins.imm_i, ins.a);
+          sv[sp] = __double_as_longlong((double)(u >> 11) * 0x1.0p-53); sn[sp] = false; ++sp;
+        } else if (op == B2_OP_RAND_I) {
+          // h > 0 (the planner's rule); a NULL or non-positive h gives NULL
+          const int64_t h = sv[sp - 1];
+          const bool ok = !sn[sp - 1] && h > 0;
+          sv[sp - 1] = ok ? (int64_t)__umul64hi(b2_rand_u64(row_base + row, ins.imm_i, ins.a), (uint64_t)h) : 0;
+          sn[sp - 1] = !ok;
         } else if (op == B2_OP_ADDMONTHS) {
           // stack: x, n
           sv[sp - 2] = b2_addmonths(sv[sp - 2], sv[sp - 1], ins.imm_i, ins.a);
@@ -359,9 +369,10 @@ int32_t b2_col_stats(const b2_col_t* col, int64_t n, int64_t* d_out, void* ws, v
   return B2_OK;
 }
 
-int32_t b2_expr_eval(const b2_prog_t* prog, const b2_col_t* cols, int32_t ncols, int64_t n,
-                     void* out_data, uint32_t* out_valid, void* stream) {
+int32_t b2_expr_eval_rows(const b2_prog_t* prog, const b2_col_t* cols, int32_t ncols, int64_t n, int64_t row_base,
+                          void* out_data, uint32_t* out_valid, void* stream) {
   B2_REQUIRE(prog && out_data, "null argument");
+  B2_REQUIRE(row_base >= 0 && (n <= 0 || n <= INT64_MAX - row_base), "row_base must be >= 0 and row_base + n fit");
   B2_REQUIRE(ncols >= 0 && ncols <= B2_MAX_COLS, "too many columns");
   B2_REQUIRE(prog->n > 0 && prog->n <= B2_MAX_PROG, "bad program length");
   // static stack-depth check so the kernel cannot run off its local stack
@@ -372,6 +383,11 @@ int32_t b2_expr_eval(const b2_prog_t* prog, const b2_col_t* cols, int32_t ncols,
       B2_REQUIRE(prog->code[i].a >= 0 && prog->code[i].a < ncols, "LOAD of unknown column");
       ++sp;
     } else if (op == B2_OP_CONST_I || op == B2_OP_CONST_F || op == B2_OP_CONST_NULL) ++sp;
+    else if (op == B2_OP_RAND_F || op == B2_OP_RAND_I) {
+      B2_REQUIRE(prog->code[i].a >= 0, "RAND: the call site a must be >= 0");
+      if (op == B2_OP_RAND_F) ++sp;
+      else B2_REQUIRE(sp >= 1, "stack underflow");
+    }
     else if (op == B2_OP_I2F || op == B2_OP_F2I || op == B2_OP_NEG_I || op == B2_OP_ABS_I ||
              op == B2_OP_NEG_F || op == B2_OP_ABS_F || op == B2_OP_SQRT_F || op == B2_OP_NOT || op == B2_OP_ISNULL_I ||
              op == B2_OP_ISNULL_F || op == B2_OP_ORD2F) { B2_REQUIRE(sp >= 1, "stack underflow"); }
@@ -417,9 +433,14 @@ int32_t b2_expr_eval(const b2_prog_t* prog, const b2_col_t* cols, int32_t ncols,
   memset(&ca, 0, sizeof(ca));
   for (int i = 0; i < ncols; ++i) ca.c[i] = cols[i];
   int grid = b2_wave_grid(b2_expr_kernel, B2_BLOCK, (n + B2_BLOCK - 1) / B2_BLOCK);
-  b2_expr_kernel<<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(*prog, ca, n, out_data, out_valid);
+  b2_expr_kernel<<<grid, B2_BLOCK, 0, (cudaStream_t)stream>>>(*prog, ca, n, row_base, out_data, out_valid);
   B2_CHECK_LAUNCH("b2_expr_kernel");
   return B2_OK;
+}
+
+int32_t b2_expr_eval(const b2_prog_t* prog, const b2_col_t* cols, int32_t ncols, int64_t n,
+                     void* out_data, uint32_t* out_valid, void* stream) {
+  return b2_expr_eval_rows(prog, cols, ncols, n, 0, out_data, out_valid, stream);
 }
 
 }  // extern "C"

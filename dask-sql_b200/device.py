@@ -338,7 +338,10 @@ def col_stats(col: DeviceColumn) -> Stats:
     return Stats(mn, mx, nulls + nans, repeat)
 
 
-def expr_eval(prog: L.Prog, cols: Sequence[DeviceColumn], n: int, want_valid: bool, out=None) -> DeviceColumn:
+def expr_eval(prog: L.Prog, cols: Sequence[DeviceColumn], n: int, want_valid: bool, out=None,
+              row_base: Optional[int] = None) -> DeviceColumn:
+    """row_base: the base-table number of row 0, which the B2_OP_RAND_* draws are keyed on (None: the
+    program draws nothing, and runs through b2_expr_eval)"""
     dev = cols[0].device if cols else cur_device()
     if out is None:
         out = torch.empty(n, dtype=_TORCH_DTYPE[prog.out_dtype], device=dev)
@@ -346,7 +349,10 @@ def expr_eval(prog: L.Prog, cols: Sequence[DeviceColumn], n: int, want_valid: bo
     arr = (L.Col * max(1, len(cols)))()
     for i, c in enumerate(cols):
         arr[i] = c.as_struct()
-    L.expr_eval(C.byref(prog), arr, len(cols), n, ptr(out), ptr(valid), stream_ptr())
+    if row_base is None:
+        L.expr_eval(C.byref(prog), arr, len(cols), n, ptr(out), ptr(valid), stream_ptr())
+    else:
+        L.expr_eval_rows(C.byref(prog), arr, len(cols), n, row_base, ptr(out), ptr(valid), stream_ptr())
     return DeviceColumn(out, valid, prog.out_dtype)
 
 

@@ -24,10 +24,11 @@ from . import _lib as L
 from . import device as D
 from . import expr as E
 from . import parallel as P
+from . import rand as R
 from . import strings as S
 from .device import DeviceColumn, TermSpec, I64, F64, U8
 from .expr import Expr, ColRef, Lit, Call
-from .frame import LazyFrame, Source, TableSource, JoinSource, AggSource, SortSource, LimitSource
+from .frame import LazyFrame, Source, TableSource, JoinSource, AggSource, SortSource, LimitSource, SAMPLE_MASK
 from .table import DeviceTable, HostColumn
 
 DENSE_MAX_SLOTS = 1 << 27          # direct-address group tables up to 128M slots
@@ -107,6 +108,9 @@ class Part(dict):
     # "replicated": every rank holds these rows (or there is one rank); "keyrange": the rows of a
     # multi-GPU aggregate, of which every rank holds the groups of its own slice of the key range
     dist = "replicated"
+    # number of row 0 in its base table (rand.py), or None for rows that have no such number: the output of
+    # a join, an aggregate, a sort, a LIMIT or a filter
+    row_base = None
 
     def __init__(self, cols=(), n=0):
         super().__init__(cols)
@@ -250,17 +254,25 @@ def simplify_pred(pred: Sequence[Expr]):
     return out, False
 
 
+RAND_RULE = ("RAND / RANDOM / RAND_INTEGER are defined on the rows of one base table only: use them in the "
+             "SELECT list, WHERE, GROUP BY or ORDER BY of a query block that reads a single table, not over the "
+             "output of a join, an aggregate, a sort or a LIMIT, whose rows have no number in a table")
+
+
 def eval_expr(part: Part, e: Expr) -> DeviceColumn:
     """Materialise expression `e` over the columns of `part` (one b2_expr_eval pass)."""
     if isinstance(e, ColRef):
         return part[e.name]
+    draws = E.has_rand(e)
+    if draws and part.row_base is None:
+        raise NotImplementedError(RAND_RULE)
     names = sorted(e.refs())
     tables = E.map_tables(e)
     cols = [part[n] for n in names] + [t.column(_dev()) for t in tables]
     prog = E.compile_expr(e, names, tables)
     nullable = E.may_be_null(e, lambda n: part[n].valid is not None)
     stats["launches"] += 1
-    out = D.expr_eval(prog, cols, part.n, nullable)
+    out = D.expr_eval(prog, cols, part.n, nullable, row_base=part.row_base if draws else None)
     out.logical = e.logical
     return out
 
@@ -505,6 +517,70 @@ def _pushdown_terms(pred) -> list:
     return out
 
 
+def table_row_start(table) -> int:
+    """Number of this rank's first row in the whole table: 0, or on a sharded table the rows of the ranks
+    before it.  That is the lower bound parallel.shard_bounds gives the rank when the shards were cut by it,
+    and it numbers every row 0 ... N-1 once whatever the shards' sizes.  The ranks' row counts are
+    all-gathered on first use (a collective: every rank asks) and kept with the immutable table."""
+    rank, world = P.world()
+    if world == 1 or table.distribution != "sharded":
+        return 0
+    if "_shard_rows" not in table.__dict__:
+        counts = [r[0] for r in P.all_gather_ints([table.nrows], _dev())]
+        table.__dict__["_shard_rows"] = counts
+        table.__dict__.setdefault("_global_nrows", sum(counts))
+    return sum(table.__dict__["_shard_rows"][:rank])
+
+
+def table_parts(src: TableSource, needed: Set[str], pred=None):
+    """[(partition {column: column}, row_base)] of a table scan: the partitions that the pushed-down conjuncts
+    and a TABLESAMPLE SYSTEM clause leave, each with the number of its first row (rand.py).  The numbers are
+    needed only by a sampled scan or one a RAND draws over (TableSource.numbered); any other scan gets
+    row_base None, and on a sharded table asks the other ranks nothing."""
+    table, sample = src.table, src.sample
+    numbered = sample is not None or src.numbered
+    start = table_row_start(table) if numbered else None
+    system = sample if sample is not None and sample.method == "system" else None
+    if hasattr(table, "scan_pruned"):
+        # lazy Parquet table: only the referenced columns of the row groups whose statistics admit
+        # a row passing the pushed-down conjuncts (conservative: the kernels still filter every row)
+        # and that SYSTEM keeps; row group g starts after the rows of groups 0 .. g-1, read or not
+        before = table.stats["row_groups_skipped"]
+        keep = None
+        if system is not None:
+            keep = [g for g in range(table.num_row_groups) if R.system_keeps(g, system.key, system.site, system.p)]
+        parts, groups = table.scan_pruned(needed, _pushdown_terms(pred), keep, with_groups=True)
+        stats["rowgroups_skipped"] = stats.get("rowgroups_skipped", 0) + table.stats["row_groups_skipped"] - before
+        if not numbered:
+            return [(p, None) for p in parts]
+        bases = R.row_bases(table.row_group_sizes(), start)
+        return [(p, start if g is None else bases[g]) for p, g in zip(parts, groups)]
+    if not numbered:
+        return [(p, None) for p in table.partitions]
+    parts = table.partitions
+    out = list(zip(parts, R.row_bases([next(iter(p.values())).n if p else 0 for p in parts], start)))
+    if system is not None:
+        out = [pb for k, pb in enumerate(out) if R.system_keeps(k, system.key, system.site, system.p)]
+        if not out:                     # nothing kept: one empty partition of the table's columns
+            out = [({n: _empty_column(c) for n, c in parts[0].items()}, start)]
+    return out
+
+
+def _empty_column(c) -> DeviceColumn:
+    return DeviceColumn(c.data[:0].to(_dev()), None, c.dtype, c.logical)
+
+
+def _sample_mask(n: int, row_base: int, sample) -> DeviceColumn:
+    """The TABLESAMPLE BERNOULLI mask of rows row_base .. row_base + n - 1 (b2_sample_mask)."""
+    out = torch.empty(n, dtype=torch.uint8, device=_dev())
+    stats["launches"] += 1
+    stats["sample_masks"] = stats.get("sample_masks", 0) + 1
+    rec = _kernel_event_begin("b2_sample_mask", n)
+    L.sample_mask(n, row_base, sample.key, sample.site, R.threshold(sample.p), D.ptr(out), D.stream_ptr())
+    _kernel_event_end(rec)
+    return DeviceColumn(out, None, U8)
+
+
 def materialize(src: Source, needed: Set[str], top: bool = False, pred=None) -> List[Part]:
     """top: the caller is the outermost frame of a query -- a multi-GPU aggregate may then stay
     sharded by key range (one slice of the groups per rank, the dask result with split_out = world
@@ -512,19 +588,13 @@ def materialize(src: Source, needed: Set[str], top: bool = False, pred=None) -> 
     if isinstance(src, TableSource):
         dev = _dev()
         parts = []
-        table = src.table
-        if hasattr(table, "scan_pruned"):
-            # lazy Parquet table: only the referenced columns of the row groups whose statistics admit
-            # a row passing the pushed-down conjuncts (conservative: the kernels still filter every row)
-            before = table.stats["row_groups_skipped"]
-            table_parts = table.scan_pruned(needed, _pushdown_terms(pred))
-            stats["rowgroups_skipped"] = stats.get("rowgroups_skipped", 0) + table.stats["row_groups_skipped"] - before
-        else:
-            table_parts = table.partitions
-        for p in table_parts:
+        for p, row_base in table_parts(src, needed, pred):
             n = next(iter(p.values())).n if p else 0
             cols = {}
             for name in needed:
+                if name == SAMPLE_MASK:
+                    cols[name] = _sample_mask(n, row_base, src.sample)
+                    continue
                 c = p[name]
                 if isinstance(c, HostColumn):
                     stats["h2d_bytes"] += c.nbytes()
@@ -533,7 +603,9 @@ def materialize(src: Source, needed: Set[str], top: bool = False, pred=None) -> 
                         # statistics ride on the first upload and stay with the (immutable) host column
                         hc.stats = c.ensure_stats()
                 cols[name] = c
-            parts.append(Part(cols, n))
+            part = Part(cols, n)
+            part.row_base = row_base
+            parts.append(part)
         return parts
     if isinstance(src, JoinSource):
         return run_join(src, needed)
@@ -752,14 +824,30 @@ def execute(frame: LazyFrame, needed: Optional[Sequence[str]] = None, top: bool 
         p.refs(src_needed)
     parts = materialize(frame.source, src_needed, top, pred)
 
+    rand_nodes = []
+    if pred:
+        for e in exprs.values():
+            E.rand_nodes(e, rand_nodes)
+
     def project(part: Part) -> Part:
         dist = part.dist
+        local = exprs
+        if rand_nodes:
+            # the filter below compacts the rows and so loses their numbers: draw first, carry the draws along
+            drawn = Part(dict(part), part.n)
+            drawn.dist, drawn.row_base = part.dist, part.row_base
+            mapping = {}
+            for i, node in enumerate(rand_nodes):
+                drawn[f"__rand{i}"] = eval_expr(part, node)
+                mapping[repr(node)] = ColRef(f"__rand{i}", node.dtype)
+            part = drawn
+            local = {n: E.replace_nodes(e, mapping) for n, e in exprs.items()}
         if pred:
-            colrefs = sorted({r for e in exprs.values() for r in e.refs()})
+            colrefs = sorted({r for e in local.values() for r in e.refs()})
             part = select_part(part, pred, colrefs)
         res = Part({}, part.n)
         res.dist = dist
-        for n, e in exprs.items():
+        for n, e in local.items():
             if isinstance(e, Lit):
                 res[n] = const_column(e.value, e.dtype, part.n, _dev())
                 res[n].logical = e.logical
@@ -2255,6 +2343,10 @@ def try_star(src: AggSource, child: LazyFrame, gexprs, aggs, pred, sharded, allo
     pk_name = js.right_on[0] if fact_side == "left" else js.left_on[0]
     if not isinstance(fact.source, TableSource):
         return None
+    if fact.source.sample is not None or (isinstance(dim.source, TableSource) and dim.source.sample is not None):
+        return None           # a sampled side takes the join-aggregate or the general join (DESIGN.md section 4)
+    if any(E.has_rand(e) for e in list(pred) + list(gexprs) + [e for e, _, _ in aggs if e is not None]):
+        return None           # the prepared star reads partitions that carry no row numbers to draw by
     fk_e, pk_e = fact.exprs[fk_name], dim.exprs[pk_name]
     if fk_e.dtype != I64 or pk_e.dtype != I64 or E.is_varchar(fk_e) or E.is_varchar(pk_e):
         return None           # string keys take the general join, which reconciles the two dictionaries
@@ -2744,7 +2836,7 @@ def count_rows(frame: LazyFrame) -> int:
     pred, never = simplify_pred(frame.pred)
     if never:
         return 0
-    if not pred and isinstance(frame.source, TableSource):
+    if not pred and isinstance(frame.source, TableSource) and frame.source.sample is None:
         return frame.source.table.nrows
     cnt = LazyFrame(AggSource(frame, [], [(None, "n", "size")])).compute()
     return int(cnt["n"].iloc[0]) if len(cnt) else 0

@@ -256,6 +256,44 @@ def math_fold(name: str, vals, digits: int = 0):
         return float(fn(*xs))
 
 
+def rand(key: int, site: int) -> Expr:
+    """RAND: a uniform DOUBLE in [0, 1) per base-table row, keyed on (key, call site) (rand.py)."""
+    return Call("rand", [], F64, param=(int(key), int(site)))
+
+
+def rand_integer(key: int, site: int, h) -> Expr:
+    """RAND_INTEGER: a BIGINT in [0, h) per base-table row, from the same draw as RAND at that call site."""
+    return Call("rand_int", [cast(as_expr(h), I64)], I64, param=(int(key), int(site)))
+
+
+def has_rand(e: Expr) -> bool:
+    """Does `e` draw per-row random numbers (so it needs its rows' numbers in the base table)?"""
+    return isinstance(e, Call) and (e.op in ("rand", "rand_int") or any(has_rand(a) for a in e.args))
+
+
+def rand_nodes(e: Expr, out=None) -> list:
+    """The distinct rand / rand_int calls of `e`, in first-use order."""
+    out = [] if out is None else out
+    if isinstance(e, Call):
+        if e.op in ("rand", "rand_int"):
+            if not any(repr(n) == repr(e) for n in out):
+                out.append(e)
+        else:
+            for a in e.args:
+                rand_nodes(a, out)
+    return out
+
+
+def replace_nodes(e: Expr, mapping: Dict[str, Expr]) -> Expr:
+    """Rewrite the sub-expressions whose repr is a key of `mapping`."""
+    r = mapping.get(repr(e))
+    if r is not None:
+        return r
+    if isinstance(e, Call):
+        return Call(e.op, [replace_nodes(a, mapping) for a in e.args], e.dtype, e.logical, e.param)
+    return e
+
+
 def case(cond, then, other) -> Expr:
     if isinstance(then, str) or isinstance(other, str):
         raise NotImplementedError("CASE with a string result: a VARCHAR value built from two sources is not "
@@ -490,6 +528,12 @@ class _Compiler:
             self.visit(args[1])
             self.emit(L.OP_ADDMONTHS, a=to_last, imm_i=tps)
             return
+        if op in ("rand", "rand_int"):
+            key, site = e.param
+            if op == "rand_int":
+                self.visit(args[0])
+            self.emit(L.OP_RAND_F if op == "rand" else L.OP_RAND_I, a=site, imm_i=key)
+            return
         if op == "map":
             k = next((i for i, t in enumerate(self.tables) if t is e.param), None)
             if k is None:
@@ -524,7 +568,7 @@ def may_be_null(e: Expr, col_nullable) -> bool:
         return e.value is None
     if e.op == "isnull":
         return False
-    if e.op in ("divt", "mod", "map", "powi"):
+    if e.op in ("divt", "mod", "map", "powi", "rand_int"):
         return True
     if e.op == "cast" and e.dtype == I64 and e.args[0].dtype == F64:
         return True

@@ -38,10 +38,21 @@ class Source:
         return ColRef(name, dt, lg)
 
 
+# the U8 column of a TABLESAMPLE BERNOULLI scan that is 1 for the rows the sample keeps (b2_sample_mask); a
+# sampled frame's first conjunct is this column, so every kernel that scans the table filters by it
+SAMPLE_MASK = "__sample__"
+
+
 class TableSource(Source):
-    def __init__(self, table):
-        self.table = table
+    """sample: the TABLESAMPLE clause on this scan of the table (rand.Sample), or None.  numbered: a RAND
+    draws over this source, so its scans carry every row's number in the table (executor.table_parts)."""
+
+    def __init__(self, table, sample=None):
+        self.table, self.sample = table, sample
+        self.numbered = False
         self.schema = OrderedDict((n, (dt, lg)) for n, dt, lg in table.schema())
+        if sample is not None and sample.method == "bernoulli":
+            self.schema[SAMPLE_MASK] = (U8, "bool")
 
 
 class JoinSource(Source):

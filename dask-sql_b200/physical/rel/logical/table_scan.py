@@ -18,11 +18,28 @@ class DaskTableScanPlugin(BaseRelPlugin):
         scan, table = rel.table_scan(), rel.getTable()
         schema, name = context.fqn(table)
         registered = context.schema[schema.lower()].tables[name.lower()]
+        if scan.sample is not None:
+            registered = self._apply_sample(registered, scan.sample, name)
         # predicates before projection: a filter column need not survive into the output
         # (table_scan.py:51-52)
         narrowed = self._apply_projections(scan, table, self._apply_filters(scan, rel, registered, context))
         names = self.fix_column_to_row_type(narrowed.column_container, rel.getRowType())
         return self.fix_dtype_to_row_type(DataContainer(narrowed.df, names), rel.getRowType())
+
+    @staticmethod
+    def _apply_sample(dc, sample, name) -> DataContainer:
+        """TABLESAMPLE (the reference's physical/rel/logical/sample.py): SYSTEM keeps whole partitions and is
+        applied where the table's partitions are read; BERNOULLI puts its row mask in front of every conjunct,
+        so each kernel that scans the table filters by it."""
+        from ....expr import ColRef, U8
+        from ....frame import LazyFrame, TableSource, SAMPLE_MASK
+        df = dc.df
+        if getattr(dc, "view", False) or not isinstance(df.source, TableSource) or df.pred:
+            raise NotImplementedError(f"TABLESAMPLE of the view {name}: only the rows of a base table have numbers "
+                                      "to sample by")
+        pred = [ColRef(SAMPLE_MASK, U8)] if sample.method == "bernoulli" else []
+        frame = LazyFrame(TableSource(df.source.table, sample), type(df.exprs)(df.exprs), pred)
+        return DataContainer(frame, dc.column_container)
 
     def _apply_filters(self, table_scan, rel, dc, context) -> DataContainer:
         """AND of every pushed-down condition (table_scan.py:101-119)."""

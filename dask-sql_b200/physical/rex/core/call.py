@@ -215,6 +215,22 @@ def _math(name):
     return run
 
 
+def _rand(name, operands, dc):
+    """RAND (operands: key, call site) and RAND_INTEGER (key, call site, h), bound by the planner from the
+    reference's RAND / RANDOM / RAND_INTEGER (call.py:809-881).  A value is drawn per base-table row, so the
+    frame must read one table: the rows of a join, an aggregate, a sort or a LIMIT have no number."""
+    from .... import expr as E
+    from ....executor import RAND_RULE
+    from ....frame import LazySeries, TableSource
+    df = getattr(dc, "df", dc)
+    if not isinstance(getattr(df, "source", None), TableSource):
+        raise NotImplementedError(RAND_RULE)
+    df.source.numbered = True
+    key, site = operands[0], operands[1]
+    e = E.rand(key, site) if name == "rand" else E.rand_integer(key, site, operands[2])
+    return LazySeries(df.source, tuple(df.pred), e)
+
+
 def _like(ilike: bool):
     """[NOT] LIKE / ILIKE with a literal pattern; the ESCAPE character defaults to a backslash, as in the
     reference (call.py:414-416)."""
@@ -302,6 +318,8 @@ class RexCallPlugin(BaseRexPlugin):
         operands = [RexConverter.convert(rel, o, dc, context=context) for o in expr.getOperands()]
         name = str(expr.getOperatorName()).lower()
         logger.debug("%s on %s", name, [str(LoggableDataFrame(o)) for o in operands])
+        if name in ("rand", "rand_integer"):
+            return _rand(name, operands, dc)
         fn = OPERATORS.get(name)
         if fn is not None:
             return fn(operands, expr)

@@ -9,7 +9,8 @@ from .sqlparse import parse_sql
 
 def plan_sql(sql, catalog, case_sensitive=True, optimize_plan=True) -> LogicalPlan:
     tree = parse_sql(sql)
-    p = Binder(sql, catalog, case_sensitive).bind_statement(tree)
-    if optimize_plan:
-        return optimize(p)
-    return bind_all(p)
+    binder = Binder(sql, catalog, case_sensitive)
+    p = binder.bind_statement(tree)
+    p = optimize(p) if optimize_plan else bind_all(p)
+    p.volatile = binder.volatile      # RAND / TABLESAMPLE without a seed: a new key every time it is planned
+    return p

@@ -3,6 +3,7 @@ src/sql.rs:586-596), for the hot-path grammar.  Produces the same plan SHAPES th
 plugins expect: Projection / Aggregate / Filter / Join / SubqueryAlias / TableScan."""
 from typing import Callable, Dict, List, Optional, Tuple
 
+from .. import rand as R
 from .. import temporal as T
 from ..utils import ParsingException
 from . import plan as P
@@ -42,6 +43,8 @@ class Binder:
                  case_sensitive: bool = True):
         """catalog(schema_or_None, table) -> (schema_name, [(column, sql_type), ...]) or None."""
         self.sql, self.catalog, self.case_sensitive = sql, catalog, case_sensitive
+        self._key = None          # the statement's key for RAND / TABLESAMPLE without a seed
+        self.volatile = False     # the statement drew that key: re-planning it must draw a new one
 
     def err(self, msg):
         raise ParsingException(self.sql, msg)
@@ -197,6 +200,8 @@ class Binder:
         if src.kind == "table":
             parts = src.name
             if len(parts) == 1 and parts[0] in ctes:
+                if src.sample is not None:
+                    self._no_sample(f"the common table expression {parts[0]}")
                 return P.SubqueryAlias(ctes[parts[0]], src.alias or parts[0])
             schema_name, table_name = (parts[-2], parts[-1]) if len(parts) >= 2 else (None, parts[0])
             found = self.catalog(schema_name, table_name)
@@ -205,8 +210,12 @@ class Binder:
             schema_name, cols = found
             fields = [RelDataTypeField(None, c, t, i) for i, (c, t) in enumerate(cols)]
             scan = P.TableScan(schema_name, table_name.lower(), table_name if not src.alias else table_name, fields)
+            if src.sample is not None:
+                scan.sample = self._bind_sample(src.sample)
             return P.SubqueryAlias(scan, src.alias) if src.alias else scan
         if src.kind == "subquery":
+            if src.sample is not None:
+                self._no_sample("a subquery")
             return P.SubqueryAlias(self.bind_query(src.query, ctes), src.alias)
         if src.kind == "join":
             left, right = self.bind_from(src.left, ctes), self.bind_from(src.right, ctes)
@@ -372,6 +381,8 @@ class Binder:
                 return PyExpr("agg", ty, name=name, args=args, distinct=e.distinct, filter=filt)
             if name in _TEMPORAL_FUNCS:
                 return self._bind_temporal(name, e.args, rec)
+            if name in _RAND_FUNCS:
+                return self._bind_rand(name, e)
             args = [rec(a) for a in e.args]
             if name == "ABS" and len(args) == 1:
                 return PyExpr("scalarfn", _norm_type(args[0].sql_type), name="abs", args=args)
@@ -379,6 +390,59 @@ class Binder:
                 return self._bind_math(name, args)
             self.err(f"Function {name} is outside the int64/float64 hot path of this layer")
         self.err(f"Unsupported expression {k}")
+
+    # -- RAND / RANDOM / RAND_INTEGER and TABLESAMPLE ------------------------------------------
+    @staticmethod
+    def _int_literal(node):
+        """the value of an integer literal node (a negated one included), else None"""
+        neg = node.kind == "neg"
+        lit = node.e if neg else node
+        if lit is None or lit.kind != "lit" or not isinstance(lit.value, int) or isinstance(lit.value, bool):
+            return None
+        return -lit.value if neg else lit.value
+
+    def _key_of(self, seed_node, what) -> int:
+        """the Philox key of a seed argument; no seed: the statement's key, drawn once per statement"""
+        if seed_node is None:
+            if self._key is None:
+                self._key, self.volatile = R.key_of(None), True
+            return self._key
+        seed = self._int_literal(seed_node)
+        if seed is None or not -2 ** 63 <= seed < 2 ** 64:
+            self.err(f"{what} takes its seed as an integer literal")
+        return R.key_of(seed)
+
+    def _bind_rand(self, name, e) -> PyExpr:
+        """RAND([seed]) / RANDOM([seed]) -> DOUBLE in [0, 1); RAND_INTEGER([seed,] h) -> BIGINT in [0, h): the
+        reference's operator table (call.py:1087-1089), keyed per call site and row (rand.py)."""
+        args = e.args
+        if name == "RAND_INTEGER":
+            if len(args) not in (1, 2):
+                self.err(f"RAND_INTEGER takes 1 or 2 argument(s), not {len(args)}")
+            h = self._int_literal(args[-1])
+            if h is None or not 0 < h < 2 ** 63:
+                self.err("RAND_INTEGER takes its bound h as a positive BIGINT literal")
+            key = self._key_of(args[0] if len(args) == 2 else None, name)
+            return PyExpr("scalarfn", "BIGINT", name="rand_integer", args=[P.lit(key), P.lit(e.site), P.lit(h)])
+        if len(args) > 1:
+            self.err(f"{name} takes 0 or 1 argument(s), not {len(args)}")
+        key = self._key_of(args[0] if args else None, name)
+        return PyExpr("scalarfn", "DOUBLE", name="rand", args=[P.lit(key), P.lit(e.site)])
+
+    def _no_sample(self, what):
+        raise NotImplementedError(f"TABLESAMPLE of {what}: only the rows of a base table have numbers to sample by")
+
+    def _bind_sample(self, node) -> R.Sample:
+        """TABLESAMPLE BERNOULLI | SYSTEM (p) [REPEATABLE (seed)]: p a numeric literal in [0, 100]"""
+        p = node.p
+        neg = p.kind == "neg"
+        lit = p.e if neg else p
+        if lit is None or lit.kind != "lit" or not isinstance(lit.value, (int, float)) or isinstance(lit.value, bool):
+            self.err("TABLESAMPLE takes its percentage as a numeric literal")
+        value = -lit.value if neg else lit.value
+        if not 0 <= value <= 100:
+            self.err(f"TABLESAMPLE percentage {value} is outside [0, 100]")
+        return R.Sample(node.method, value, self._key_of(node.seed, "TABLESAMPLE ... REPEATABLE"), node.site)
 
     # -- numeric functions --------------------------------------------------------------------
     def _bind_math(self, name, args) -> PyExpr:
@@ -469,6 +533,7 @@ class Binder:
         return PyExpr("scalarfn", "BIGINT", name="timestampdiff", args=[P.lit(unit), a, b])
 
 
+_RAND_FUNCS = ("RAND", "RANDOM", "RAND_INTEGER")
 _TEMPORAL_FUNCS = ("EXTRACT", "DATE_PART", "DATEPART", "YEAR", "TIMESTAMPADD", "TIMESTAMPDIFF", "TIMESTAMPFLOOR",
                    "TIMESTAMPCEIL", "LAST_DAY")
 _MATH_UNARY = ("CEIL", "FLOOR", "TRUNCATE", "ROUND", "SIGN", "DEGREES", "RADIANS", "SQRT", "EXP", "LN", "LOG10", "CBRT",

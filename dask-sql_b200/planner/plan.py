@@ -437,6 +437,7 @@ class TableScan(LogicalPlan):
         self.projection_names: Optional[List[str]] = None
         self.filters: List[PyExpr] = []
         self.schema = list(self.all_fields)
+        self.sample = None        # TABLESAMPLE clause (rand.Sample)
 
     def set_projection(self, names: Optional[List[str]]):
         self.projection_names = names

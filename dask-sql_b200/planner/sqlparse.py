@@ -7,7 +7,7 @@ that crate cannot be built here (no rustc/cargo), so this is a small recursive-d
   SELECT [DISTINCT] item [, ...] FROM source [join ...] [WHERE e] [GROUP BY e, ...] [HAVING e]
   [ORDER BY e [ASC|DESC] [NULLS FIRST|LAST], ...] [LIMIT n [OFFSET m]]
 
-  source := table [[AS] alias] | ( select ) [AS] alias
+  source := table [[AS] alias] [TABLESAMPLE BERNOULLI | SYSTEM (p) [REPEATABLE (seed)]] | ( select ) [AS] alias
   join   := [INNER | LEFT [OUTER] | RIGHT [OUTER] | FULL [OUTER] | CROSS] JOIN source [ON e]
 
 Expressions: literals (incl. DATE '...', TIMESTAMP '...', INTERVAL '...' [unit]), [qualifier.]column,
@@ -21,8 +21,11 @@ Statements around the path (custom statements of the reference's parser, src/par
   CREATE [OR REPLACE] TABLE [IF NOT EXISTS] [schema.]name WITH (key = literal [, ...])
   DROP TABLE [IF EXISTS] [schema.]name
   ANALYZE TABLE [schema.]name COMPUTE STATISTICS FOR ALL COLUMNS | COLUMNS c1 [, c2 ...]
-CREATE / DROP / TABLE / VIEW / IF / EXISTS / REPLACE / ANALYZE / COMPUTE / STATISTICS / FOR / COLUMNS are
-contextual words, not reserved.
+CREATE / DROP / TABLE / VIEW / IF / EXISTS / REPLACE / ANALYZE / COMPUTE / STATISTICS / FOR / COLUMNS and
+TABLESAMPLE / BERNOULLI / SYSTEM / REPEATABLE are contextual words, not reserved.
+
+Every RAND / RANDOM / RAND_INTEGER call and every TABLESAMPLE clause gets its call-site number `site`
+(1, 2, 3 ... in textual order), which keys its random numbers apart from the statement's other ones.
 """
 import re
 from typing import List, Optional
@@ -45,6 +48,7 @@ KEYWORDS = {"SELECT", "FROM", "WHERE", "GROUP", "BY", "HAVING", "ORDER", "LIMIT"
 
 
 _LIKE_WORDS = ("LIKE", "ILIKE", "SIMILAR")
+RAND_FUNCS = ("RAND", "RANDOM", "RAND_INTEGER")
 _STRING_FUNCS = {"CONCAT", "UPPER", "LOWER", "SUBSTRING", "SUBSTR", "TRIM", "LTRIM", "RTRIM", "BTRIM", "POSITION",
                  "STRPOS", "CHAR_LENGTH", "CHARACTER_LENGTH", "LENGTH", "REPLACE", "INITCAP", "OVERLAY"}
 _TIME_UNITS = {"YEAR", "QUARTER", "MONTH", "WEEK", "DAY", "HOUR", "MINUTE", "SECOND", "MILLISECOND", "MICROSECOND",
@@ -97,6 +101,7 @@ class Parser:
         self.sql = sql
         self.toks = tokenize(sql)
         self.i = 0
+        self.sites = 0           # call sites of RAND / TABLESAMPLE numbered so far
 
     # -- helpers
     @property
@@ -370,16 +375,40 @@ class Parser:
             self.expect_op(")")
             self.eat_kw("AS")
             alias = self.ident()
-            return Node("subquery", query=q, alias=alias)
+            return Node("subquery", query=q, alias=alias, sample=self.parse_tablesample())
         parts = [self.ident()]
         while self.eat_op("."):
             parts.append(self.ident())
         alias = None
         if self.eat_kw("AS"):
             alias = self.ident()
-        elif self.cur.kind == "id":
+        elif self.cur.kind == "id" and not self.at_tablesample():
             alias = self.ident()
-        return Node("table", name=parts, alias=alias)
+        return Node("table", name=parts, alias=alias, sample=self.parse_tablesample())
+
+    def at_tablesample(self):
+        if not self.at_word("TABLESAMPLE"):
+            return False
+        nxt = self.toks[self.i + 1]
+        return nxt.kind == "id" and nxt.val.upper() in ("BERNOULLI", "SYSTEM")
+
+    def parse_tablesample(self) -> Optional[Node]:
+        """TABLESAMPLE BERNOULLI | SYSTEM (p) [REPEATABLE (seed)]; p and seed are checked by the binder"""
+        if not self.at_tablesample():
+            return None
+        self.i += 1
+        method = self.eat_word("BERNOULLI", "SYSTEM").lower()
+        self.sites += 1
+        site = self.sites
+        self.expect_op("(")
+        p = self.parse_expr()
+        self.expect_op(")")
+        seed = None
+        if self.eat_word("REPEATABLE"):
+            self.expect_op("(")
+            seed = self.parse_expr()
+            self.expect_op(")")
+        return Node("tablesample", method=method, p=p, seed=seed, site=site)
 
     # -- expressions (precedence climbing)
     def parse_expr(self) -> Node:
@@ -557,6 +586,17 @@ class Parser:
         if t.kind == "id" or (t.kind == "kw" and t.val in ("LEFT", "RIGHT", "FIRST", "LAST", "FILTER")
                               and self.toks[self.i + 1].kind == "op" and self.toks[self.i + 1].val in ("(", ".")):
             name = self.ident() if t.kind == "id" else (self.toks[self.i].val, setattr(self, "i", self.i + 1))[0]
+            if name.upper() in RAND_FUNCS and self.at_op("("):
+                self.sites += 1
+                site = self.sites
+                self.i += 1
+                args = []
+                if not self.at_op(")"):
+                    args.append(self.parse_expr())
+                    while self.eat_op(","):
+                        args.append(self.parse_expr())
+                self.expect_op(")")
+                return Node("func", name=name.upper(), args=args, distinct=False, star=False, filter=None, site=site)
             if self.eat_op("("):  # function call
                 distinct = bool(self.eat_kw("DISTINCT"))
                 args, star = [], False

@@ -430,7 +430,7 @@ class ParquetTable(DeviceTable):
                     cols[nm] = None
             self._groups.append({"rows": rg.num_rows, "cols": cols})
         self._cache = {}                        # (row group, column) -> HostColumn
-        self.stats = {"scans": 0, "row_groups_read": 0, "row_groups_skipped": 0}
+        self.stats = {"scans": 0, "row_groups_read": 0, "row_groups_skipped": 0, "row_groups_sampled_out": 0}
         S.check_distribution(distribution, [(n, None, lg) for n, lg in self._varchar.items()])
         self.distribution = distribution
         self.name = name
@@ -530,15 +530,30 @@ class ParquetTable(DeviceTable):
                 keep.append(g)
         return keep
 
-    def scan_pruned(self, needed, terms):
-        """[{column: HostColumn}] for the row groups that survive `terms`, restricted to `needed`"""
+    @property
+    def num_row_groups(self):
+        return len(self._groups)
+
+    def row_group_sizes(self):
+        """rows of every row group, from the footer"""
+        return [g["rows"] for g in self._groups]
+
+    def scan_pruned(self, needed, terms, sampled=None, with_groups=False):
+        """[{column: HostColumn}] for the row groups that survive `terms`, restricted to `needed`.
+        sampled: the row groups a TABLESAMPLE SYSTEM clause keeps (None: all); the others are never read.
+        with_groups: also return each partition's row group (None for the empty stand-in partition)."""
         keep = self.surviving_groups(terms)
+        if sampled is not None:
+            sampled = set(sampled)
+            self.stats["row_groups_sampled_out"] += sum(g not in sampled for g in keep)
+            keep = [g for g in keep if g in sampled]
         self.stats["scans"] += 1
         self.stats["row_groups_read"] += len(keep)
         self.stats["row_groups_skipped"] += len(self._groups) - len(keep)
         cols = [n for n in self._names if n in needed]
-        parts = [{n: self._column(g, n) for n in cols} for g in keep if self._groups[g]["rows"] > 0]
+        groups = [g for g in keep if self._groups[g]["rows"] > 0]
+        parts = [{n: self._column(g, n) for n in cols} for g in groups]
         if not parts:
             proto = self._prototype()
-            parts = [{n: proto[n] for n in cols}]
-        return parts
+            parts, groups = [{n: proto[n] for n in cols}], [None]
+        return (parts, groups) if with_groups else parts

@@ -210,6 +210,11 @@ typedef struct b2_prog {
                                power of ten f; imm_i = 0: rint(x * f) / f, imm_i = 1: rint(x / f) * f */
 #define B2_OP_MATH2_F   64  /* pops y, x, pushes function a (B2_FN_ATAN2 .. B2_FN_MOD) of (x, y) */
 #define B2_OP_POW_I     65  /* pops y, x: x ** y on int64, wrapping modulo 2^64 (np.power); y < 0 -> NULL */
+/* RAND / RANDOM / RAND_INTEGER (the reference's physical/rex/core/call.py:809-881, re-keyed): for row r =
+ * row_base (b2_expr_eval_rows) + the row's index, u = w0 | w1 << 32 of Philox4x32-10 with counter (r mod 2^32, r >> 32, a, 0)
+ * and key (imm_i low word, imm_i high word); a is the call site (>= 0).  DESIGN.md section 3. */
+#define B2_OP_RAND_F    66  /* pushes (u >> 11) * 2^-53, a double in [0, 1) */
+#define B2_OP_RAND_I    67  /* pops h, pushes (u * h) >> 64, an int64 in [0, h); NULL or h <= 0 -> NULL */
 #define B2_FN_CEIL     0   /* np.ceil */
 #define B2_FN_FLOOR    1   /* np.floor */
 #define B2_FN_TRUNC    2   /* np.trunc */
@@ -261,6 +266,19 @@ int32_t b2_col_stats(const b2_col_t* col, int64_t n, int64_t* d_out, void* ws, v
  * out_valid != NULL, the Arrow validity bitmap of the result ((n+31)/32 uint32 words). */
 int32_t b2_expr_eval(const b2_prog_t* prog, const b2_col_t* cols, int32_t ncols, int64_t n,
                      void* out_data, uint32_t* out_valid, void* stream);
+/* b2_expr_eval over rows numbered row_base, row_base + 1, ... in their base table: the counter of the
+ * B2_OP_RAND_* draws.  b2_expr_eval is this with row_base = 0. */
+int32_t b2_expr_eval_rows(const b2_prog_t* prog, const b2_col_t* cols, int32_t ncols, int64_t n, int64_t row_base,
+                          void* out_data, uint32_t* out_valid, void* stream);
+
+/* ---- TABLESAMPLE BERNOULLI ----------------------------------------------------------- */
+/* The reference samples per dask partition with a seeded RandomState (physical/rel/logical/sample.py); here
+ * the choice is keyed on the row's number in its table.  out[i] = 1 iff row r = row_base + i is kept: with
+ * g = r >> 2 and w = Philox4x32-10(counter (g mod 2^32, g >> 32, site, 1), key (key low, key high)), iff
+ * w[r & 3] < threshold.  threshold = round(p / 100 * 2^32); <= 0 keeps no row and >= 2^32 every row, without
+ * drawing.  One Philox call per group of four rows; a group may straddle two partitions. */
+int32_t b2_sample_mask(int64_t n, int64_t row_base, int64_t key, int32_t site, int64_t threshold, uint8_t* out,
+                       void* stream);
 
 /* ---- VARCHAR dictionaries ---------------------------------------------------------- */
 /* A VARCHAR column is int64 codes into a dictionary sorted by UTF-8 bytes (so code order is string

@@ -177,6 +177,19 @@ def main():
                     assert (pd.isna(a) and pd.isna(b)) or abs(a - b) <= 1e-9 * max(1.0, abs(b)), (col, row, a, b)
                 else:
                     assert (pd.isna(a) and pd.isna(b)) or a == b, (col, row, a, b)
+    # 7. RAND and TABLESAMPLE BERNOULLI on a sharded table: rank r numbers its rows from the rows of the ranks
+    # before it, so the ranks' rows together are the sample and the column one GPU computes -- on the table cut
+    # by shard_bounds, and on one cut unevenly (rank r holding a share proportional to r + 1)
+    sql = "SELECT skey, gk, RAND(7) AS r FROM {} TABLESAMPLE BERNOULLI (10) REPEATABLE (3) WHERE x > 0"
+    weights = np.cumsum([0] + [r + 1 for r in range(world)])
+    ulo, uhi = (int(nf * weights[rank] // weights[-1]), int(nf * weights[rank + 1] // weights[-1]))
+    c.create_table("fact_u", fact.iloc[ulo:uhi], persist=True, npartitions=2, distribution="sharded")
+    one = c5.sql(sql.format("fact")).compute()
+    for name in ("fact", "fact_u"):
+        got = c.sql(sql.format(name)).compute()
+        parts = [None] * world
+        dist.all_gather_object(parts, got)
+        check(pd.concat(parts, ignore_index=True), one, ["skey", "gk", "r"], [])
     dist.barrier()
     if rank == 0:
         print(f"mgpu_check OK on {world} GPUs")
