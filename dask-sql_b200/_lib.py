@@ -98,6 +98,26 @@ PEER_PRESENT_ROWS, PEER_PRESENT_INDICATOR, PEER_PRESENT_BITMAP = 1, 2, 3
 SELECT_MAX_TARGETS, SELECT_MAX_BITS = 8, 11
 
 
+class WinPrefix(C.Structure):
+    _fields_ = [("val", C.c_void_p), ("lo", C.c_void_p), ("cnt", C.c_void_p), ("pinf", C.c_void_p),
+                ("ninf", C.c_void_p)]
+
+
+class WinFrame(C.Structure):
+    _fields_ = [("fn", C.c_int32), ("range", C.c_int32), ("lo", C.c_int64), ("hi", C.c_int64), ("n", C.c_int64),
+                ("ps", C.c_void_p), ("qs", C.c_void_p), ("dn", C.c_void_p), ("pend", C.c_void_p),
+                ("qend", C.c_void_p), ("val", Col), ("pre", WinPrefix), ("suf", WinPrefix), ("peer", WinPrefix),
+                ("rmq", C.c_void_p), ("rmq_levels", C.c_int32), ("pad_", C.c_int32), ("out", C.c_void_p),
+                ("out_valid", C.c_void_p)]
+
+
+# window scans and functions (b200sql.h B2_WIN_* / B2_WF_*)
+WIN_SUM_I, WIN_SUM_F, WIN_MIN, WIN_MAX = range(4)
+WIN_UNBOUNDED = 1 << 40
+(WF_ROW_NUMBER, WF_RANK, WF_DENSE_RANK, WF_COUNT_STAR, WF_COUNT, WF_SUM_I, WF_SUM_F, WF_AVG, WF_MIN, WF_MAX,
+ WF_FIRST_VALUE, WF_LAST_VALUE) = range(12)
+
+
 class Select(C.Structure):
     _fields_ = [("prefix", C.c_uint64 * SELECT_MAX_TARGETS), ("nsel", C.c_int32), ("shift", C.c_int32),
                 ("bits", C.c_int32), ("pad_", C.c_int32)]
@@ -229,12 +249,18 @@ _SIGS = {
                           C.POINTER(AggState), _P, _P],
     "b2_star_build_pack": [_P, C.c_int64, _P, C.c_int64, _P, C.c_int32, _P],
     "b2_sample_mask": [C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int64, _P, _P],
+    "b2_window_heads": [C.POINTER(Col), _P, C.c_int64, C.c_int32, _P, _P],
+    "b2_window_positions": [_P, C.c_int64, _P, _P, _P, _P, _P, _P, _P],
+    "b2_window_scan": [_P, C.POINTER(Col), C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.POINTER(WinPrefix), _P, _P],
+    "b2_window_rmq": [C.POINTER(Col), C.c_int64, C.c_int32, C.c_int32, _P, _P],
+    "b2_window_frame": [C.POINTER(WinFrame), _P],
+    "b2_window_invert": [_P, C.c_int64, _P, _P],
     "b2_str_like": [_P, _P, C.c_int64, _P, C.c_int64, C.c_uint32, C.c_int32, _P, _P],
     "b2_str_lower_bound": [_P, _P, C.c_int64, _P, _P, C.c_int64, C.c_int32, _P, _P, _P],
 }
 
 EXPORTS = sorted(list(_SIGS) + ["b2_last_error", "b2_num_tiles", "b2_stats_ws_bytes", "b2_scan_agg_ws_bytes",
-                                "b2_sort_ws_bytes", "b2_range_partition_ws_bytes",
+                                "b2_sort_ws_bytes", "b2_range_partition_ws_bytes", "b2_window_ws_bytes",
                                 "b2_f64_to_ordered", "b2_ordered_to_f64"])
 
 
@@ -329,6 +355,15 @@ star_agg_narrow = _wrap("b2_star_agg_narrow")
 star_agg_multi = _wrap("b2_star_agg_multi")
 star_build_pack = _wrap("b2_star_build_pack")
 sample_mask = _wrap("b2_sample_mask")
+window_heads = _wrap("b2_window_heads")
+window_positions = _wrap("b2_window_positions")
+window_scan = _wrap("b2_window_scan")
+window_rmq = _wrap("b2_window_rmq")
+window_frame = _wrap("b2_window_frame")
+window_invert = _wrap("b2_window_invert")
+_lib.b2_window_ws_bytes.restype = C.c_int64
+_lib.b2_window_ws_bytes.argtypes = [C.c_int64]
+window_ws_bytes = _lib.b2_window_ws_bytes
 str_like = _wrap("b2_str_like")
 str_lower_bound = _wrap("b2_str_lower_bound")
 num_tiles = _lib.b2_num_tiles

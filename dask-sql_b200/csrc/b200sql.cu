@@ -38,6 +38,7 @@ int b2_sm_count() {
 #include "join.cuh"
 #include "joinagg.cuh"
 #include "sort.cuh"
+#include "window.cuh"
 #include "select.cuh"
 #include "partition.cuh"
 #include "peer.cuh"

@@ -11,20 +11,28 @@
 #define B2_SORT_ITEMS_PER_WARP 2048   // rows of one warp's contiguous sub-chunk
 #define B2_SORT_CHUNK (B2_SORT_WARPS * B2_SORT_ITEMS_PER_WARP)
 
+// ascending unsigned image of col[r] for the sort order, and whether the row is NULL (NaN for floats).
+// Two rows sort as equals exactly when both are NULL or both are non-NULL with equal images; the window
+// kernels (window.cuh) take partitions and peer groups from the same rule.
+__device__ __forceinline__ uint64_t b2_sort_key_image(const b2_col_t& c, int64_t r, bool& isnull) {
+  int64_t raw = c.dtype == B2_U8 ? (int64_t) reinterpret_cast<const uint8_t*>(c.data)[r]
+                                 : __ldg(reinterpret_cast<const long long*>(c.data) + r);
+  isnull = b2_is_null(c, r, raw);
+  if (c.dtype == B2_F64) {
+    if (raw == (int64_t)0x8000000000000000LL) raw = 0;  // -0.0 sorts with 0.0
+    raw = b2_ordered_from_bits(raw);
+  }
+  return (uint64_t)raw ^ 0x8000000000000000ULL;  // signed -> unsigned order
+}
+
 // image of col[src row] for the sort order; out_null[i] = 1 for NULL rows (NaN for floats)
 __global__ void __launch_bounds__(B2_BLOCK)
 b2_sort_image_kernel(const __grid_constant__ b2_col_t c, const int32_t* __restrict__ idx, int64_t n, int descending,
                      int nulls_first, uint64_t* __restrict__ out_img, uint8_t* __restrict__ out_null) {
   for (int64_t i = (int64_t)blockIdx.x * B2_BLOCK + threadIdx.x; i < n; i += (int64_t)gridDim.x * B2_BLOCK) {
     const int64_t r = idx ? idx[i] : i;
-    int64_t raw = c.dtype == B2_U8 ? (int64_t) reinterpret_cast<const uint8_t*>(c.data)[r]
-                                   : __ldg(reinterpret_cast<const long long*>(c.data) + r);
-    const bool isnull = b2_is_null(c, r, raw);
-    if (c.dtype == B2_F64) {
-      if (raw == (int64_t)0x8000000000000000LL) raw = 0;  // -0.0 sorts with 0.0
-      raw = b2_ordered_from_bits(raw);
-    }
-    uint64_t img = (uint64_t)raw ^ 0x8000000000000000ULL;  // signed -> unsigned order
+    bool isnull;
+    uint64_t img = b2_sort_key_image(c, r, isnull);
     if (descending) img = ~img;
     out_img[i] = isnull ? 0 : img;
     // most significant digit: 0 sorts first.  NULLS FIRST -> NULL rows get 0, others 1 (and vice versa)

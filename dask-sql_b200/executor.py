@@ -28,7 +28,8 @@ from . import rand as R
 from . import strings as S
 from .device import DeviceColumn, TermSpec, I64, F64, U8
 from .expr import Expr, ColRef, Lit, Call
-from .frame import LazyFrame, Source, TableSource, JoinSource, AggSource, SortSource, LimitSource, SAMPLE_MASK
+from .frame import (LazyFrame, Source, TableSource, JoinSource, AggSource, SortSource, LimitSource, WindowSource,
+                    SAMPLE_MASK)
 from .table import DeviceTable, HostColumn
 
 DENSE_MAX_SLOTS = 1 << 27          # direct-address group tables up to 128M slots
@@ -618,6 +619,8 @@ def materialize(src: Source, needed: Set[str], top: bool = False, pred=None) -> 
         return [run_sort(src, needed)]
     if isinstance(src, LimitSource):
         return [run_limit(src, needed)]
+    if isinstance(src, WindowSource):
+        return [run_window(src, needed)]
     raise TypeError(f"unknown source {type(src).__name__}")
 
 
@@ -642,6 +645,182 @@ def run_sort(src: SortSource, needed: Set[str]) -> Part:
         if k in needed:
             stats["launches"] += 1
             out[k] = D.gather(whole[k], idx, False)
+    return out
+
+
+WINDOW_MAX_ROWS = (1 << 31) - 1      # sorted positions are int32
+_WF = {"row_number": L.WF_ROW_NUMBER, "rank": L.WF_RANK, "dense_rank": L.WF_DENSE_RANK, "count": L.WF_COUNT,
+       "min": L.WF_MIN, "max": L.WF_MAX, "first_value": L.WF_FIRST_VALUE, "last_value": L.WF_LAST_VALUE}
+
+
+def window_refusal(child: LazyFrame) -> Optional[str]:
+    """Why the rows of `child` cannot take window functions here, or None."""
+    if P.world()[1] > 1 and frame_distribution(child) in ("sharded", "root"):
+        return ("window functions over a sharded or root table on more than one GPU: a partition's rows would "
+                "have to meet on one rank first")
+    if estimated_rows(child) > WINDOW_MAX_ROWS:
+        return f"window functions over more than {WINDOW_MAX_ROWS} rows"
+    return None
+
+
+def _window_bound(b) -> int:
+    if b == float("-inf"):
+        return -L.WIN_UNBOUNDED
+    if b == float("inf"):
+        return L.WIN_UNBOUNDED
+    return max(-(1 << 32), min(1 << 32, int(b)))
+
+
+class _WindowSpecRun:
+    """One (PARTITION BY, ORDER BY) spec over the rows of `whole`: the sort, the heads and positions, and the
+    scans its functions share (b2_sort_by, b2_window_*)."""
+
+    def __init__(self, whole: Part, partition, order):
+        self.whole, n, dev, st = whole, whole.n, _dev(), D.stream_ptr()
+        self.n, self.dev = n, dev
+        rec = _kernel_event_begin("window_sort", n)
+        self.idx = torch.empty(n, dtype=torch.int32, device=dev)
+        L.iota(D.ptr(self.idx), n, st)
+        keys = [(k, True, False) for k in partition] + list(order)
+        if keys:
+            ws = torch.empty(L.sort_ws_bytes(n), dtype=torch.uint8, device=dev)
+            for name, asc, nulls_first in reversed(keys):
+                cs = whole[name].as_struct()
+                stats["launches"] += 29
+                L.sort_by(C.byref(cs), n, 0 if asc else 1, 1 if nulls_first else 0, D.ptr(self.idx), D.ptr(ws), st)
+            del ws
+        _kernel_event_end(rec)
+        rec = _kernel_event_begin("window_kernels", n)
+        self.flags = torch.zeros(n, dtype=torch.uint8, device=dev)
+        self.flags[:1] = 3
+        for names, is_part in ((partition, 1), ([k for k, _, _ in order], 0)):
+            for name in names:
+                cs = whole[name].as_struct()
+                stats["launches"] += 1
+                L.window_heads(C.byref(cs), D.ptr(self.idx), n, is_part, D.ptr(self.flags), st)
+        self.ws = torch.empty(L.window_ws_bytes(n), dtype=torch.uint8, device=dev)
+        self.pos = [torch.empty(n, dtype=torch.int32, device=dev) for _ in range(5)]   # ps, qs, dn, pend, qend
+        stats["launches"] += 3
+        L.window_positions(D.ptr(self.flags), n, *(D.ptr(t) for t in self.pos), D.ptr(self.ws), st)
+        _kernel_event_end(rec)
+        self.sorted, self.scans = {}, {}
+
+    def sorted_arg(self, name) -> DeviceColumn:
+        if name not in self.sorted:
+            rec = _kernel_event_begin("window_kernels", self.n)
+            stats["launches"] += 1
+            self.sorted[name] = D.gather(self.whole[name], self.idx, False)
+            _kernel_event_end(rec)
+        return self.sorted[name]
+
+    def scan(self, name, kind, seg_mask=1, reverse=0):
+        """(b2_win_prefix_t, the tensors behind it) of one scan of a sorted argument, computed once"""
+        key = (name, kind, seg_mask, reverse)
+        if key not in self.scans:
+            val = self.sorted_arg(name)
+            n, dev = self.n, self.dev
+            t = {"val": torch.empty(n, dtype=torch.float64 if kind == L.WIN_SUM_F else torch.int64, device=dev),
+                 "cnt": torch.empty(n, dtype=torch.int32, device=dev)}
+            if kind == L.WIN_SUM_F:
+                t["lo"] = torch.empty(n, dtype=torch.float64, device=dev)
+                t["pinf"] = torch.empty(n, dtype=torch.int32, device=dev)
+                t["ninf"] = torch.empty(n, dtype=torch.int32, device=dev)
+            pre = L.WinPrefix(**{k: D.ptr(v).value for k, v in t.items()})
+            cs = val.as_struct()
+            rec = _kernel_event_begin("window_kernels", n)
+            stats["launches"] += 3
+            L.window_scan(D.ptr(self.flags), C.byref(cs), n, kind, seg_mask, reverse, C.byref(pre), D.ptr(self.ws),
+                          D.stream_ptr())
+            _kernel_event_end(rec)
+            self.scans[key] = (pre, t)
+        return self.scans[key][0]
+
+    def function(self, fn, arg, frame) -> DeviceColumn:
+        """one window function, in sorted order"""
+        n, dev = self.n, self.dev
+        is_range, lo, hi = frame
+        f = L.WinFrame()
+        f.range, f.lo, f.hi, f.n = int(bool(is_range)), _window_bound(lo), _window_bound(hi), n
+        f.ps, f.qs, f.dn, f.pend, f.qend = (D.ptr(t).value for t in self.pos)
+        out_dt, logical = I64, "int64"
+        if arg is not None:
+            val = self.sorted_arg(arg)
+            f.val = val.as_struct()
+        if fn == "count":
+            f.fn = L.WF_COUNT_STAR if arg is None else L.WF_COUNT
+            if arg is not None:
+                f.pre = self.scan(arg, L.WIN_SUM_I)
+        elif fn in ("sum", "avg"):
+            is_f = fn == "avg" or val.dtype == F64
+            f.fn = L.WF_AVG if fn == "avg" else L.WF_SUM_F if is_f else L.WF_SUM_I
+            f.pre = self.scan(arg, L.WIN_SUM_F if is_f else L.WIN_SUM_I)
+            out_dt, logical = (F64, "float64") if is_f else (I64, "int64")
+        elif fn in ("min", "max"):
+            f.fn = _WF[fn]
+            kind = L.WIN_MIN if fn == "min" else L.WIN_MAX
+            f.pre = self.scan(arg, kind)
+            if f.hi >= L.WIN_UNBOUNDED and f.lo > -L.WIN_UNBOUNDED:
+                f.suf = self.scan(arg, kind, 1, 1)
+            if f.range and f.lo == 0 and f.hi == 0:
+                f.peer = self.scan(arg, kind, 2)
+            if not f.range and f.lo > -L.WIN_UNBOUNDED and f.hi < L.WIN_UNBOUNDED and f.hi >= f.lo:
+                levels = max(1, min(n, f.hi - f.lo + 1).bit_length())
+                table = torch.empty(levels * n, dtype=torch.int64, device=dev)
+                cs = val.as_struct()
+                rec = _kernel_event_begin("window_kernels", n)
+                stats["launches"] += levels
+                L.window_rmq(C.byref(cs), n, 1 if fn == "max" else 0, levels, D.ptr(table), D.stream_ptr())
+                _kernel_event_end(rec)
+                f.rmq, f.rmq_levels = D.ptr(table).value, levels   # freed behind the launch, as run_sort's ws
+            out_dt, logical = (val.dtype, val.logical) if val.dtype != U8 else (I64, "int64")
+        else:
+            f.fn = _WF[fn]
+            if arg is not None:
+                out_dt, logical = val.dtype, val.logical
+        out = torch.empty(n, dtype=_TORCH_DT[out_dt], device=dev)
+        nullable = fn not in ("row_number", "rank", "dense_rank", "count")
+        valid = torch.empty(D.bitmap_words(n), dtype=torch.int32, device=dev) if nullable else None
+        f.out, f.out_valid = D.ptr(out).value, D.ptr(valid).value
+        rec = _kernel_event_begin("window_kernels", n)
+        stats["launches"] += 1
+        L.window_frame(C.byref(f), D.stream_ptr())
+        _kernel_event_end(rec)
+        return DeviceColumn(out, valid, out_dt, logical)
+
+
+def run_window(src: WindowSource, needed: Set[str]) -> Part:
+    """Window functions: per (PARTITION BY, ORDER BY) spec one stable sort of row ids (b2_sort_by per key, last
+    key first, as run_sort), the heads and positions, the scans its functions share, one b2_window_frame per
+    function, and a gather of each result back to input row order (b2_window_invert + b2_gather)."""
+    why = window_refusal(src.child)
+    if why is not None:
+        raise NotImplementedError(why)
+    inputs = src.inputs()
+    names = [n for n in src.child.columns if n in needed or n in inputs]
+    whole = concat_parts(execute(src.child, names), names)
+    n = whole.n
+    if n > WINDOW_MAX_ROWS:
+        raise NotImplementedError(f"window functions over more than {WINDOW_MAX_ROWS} rows")
+    out = Part({k: whole[k] for k in names if k in needed}, n)
+    dev = _dev()
+    for partition, order, funcs in src.specs:
+        wanted = [(o, fn, a, fr) for o, fn, a, fr in funcs if o in needed]
+        if not wanted:
+            continue
+        if n == 0:
+            for o, fn, a, _ in wanted:
+                dt, lg = src.schema[o]
+                out[o] = DeviceColumn(torch.empty(0, dtype=_TORCH_DT[dt], device=dev), None, dt, lg)
+            continue
+        run = _WindowSpecRun(whole, partition, order)
+        results = [(o, run.function(fn, a, fr)) for o, fn, a, fr in wanted]
+        rec = _kernel_event_begin("window_scatter", n)
+        inv = torch.empty(n, dtype=torch.int32, device=dev)
+        stats["launches"] += 1 + len(results)
+        L.window_invert(D.ptr(run.idx), n, D.ptr(inv), D.stream_ptr())
+        for o, col in results:
+            out[o] = D.gather(col, inv, False)
+        _kernel_event_end(rec)
     return out
 
 

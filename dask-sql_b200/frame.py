@@ -113,6 +113,45 @@ class SortSource(Source):
         self.schema = OrderedDict((n, child.col_type(n)) for n in child.columns)
 
 
+WINDOW_FUNCS = ("row_number", "rank", "dense_rank", "count", "sum", "avg", "min", "max", "first_value", "last_value")
+
+
+class WindowSource(Source):
+    """Window functions over the child's rows, output in the child's row order.  specs: one entry per distinct
+    (PARTITION BY, ORDER BY): (partition columns, order keys [(column, ascending, nulls_first)], functions
+    [(output column, fn, argument column or None, frame)]); fn is one of WINDOW_FUNCS, "count" without an
+    argument is COUNT(*).  frame = (is_range, lo, hi): bounds relative to the row, -k for k PRECEDING, 0 for
+    CURRENT ROW, +k for k FOLLOWING, -inf / +inf for UNBOUNDED; a RANGE frame takes only 0 and +-inf."""
+
+    def __init__(self, child: "LazyFrame", specs):
+        self.child, self.specs = child, [(list(p), list(o), list(f)) for p, o, f in specs]
+        self.schema = OrderedDict((n, child.col_type(n)) for n in child.columns)
+        for _, _, funcs in self.specs:
+            for out, fn, arg, _ in funcs:
+                self.schema[out] = self._result_type(fn, arg)
+
+    def _result_type(self, fn, arg):
+        if fn in ("row_number", "rank", "dense_rank", "count"):
+            return I64, "int64"
+        dt, lg = self.child.col_type(arg)
+        if fn == "avg":
+            return F64, "float64"
+        if fn in ("first_value", "last_value"):
+            return dt, lg
+        if dt == U8:
+            return I64, "int64"
+        if fn == "sum":
+            return (F64, "float64") if dt == F64 else (I64, "int64")
+        return dt, lg                       # MIN / MAX keep a VARCHAR's dictionary and a DATE's type
+
+    def inputs(self):
+        """the child columns the window reads: keys and arguments"""
+        out = []
+        for part, order, funcs in self.specs:
+            out += list(part) + [k for k, _, _ in order] + [a for _, _, a, _ in funcs if a is not None]
+        return list(dict.fromkeys(out))
+
+
 class LimitSource(Source):
     """LIMIT / OFFSET over the child's row order."""
 

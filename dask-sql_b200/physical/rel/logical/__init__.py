@@ -1,6 +1,6 @@
 """Plan-node plugins of the filter -> join -> group-by path and the operators either side of it."""
 from . import (aggregate, cross_join, empty, explain, filter, join, limit, project, sort,  # noqa: A004
-               subquery_alias, table_scan)
+               subquery_alias, table_scan, window)
 
 DaskTableScanPlugin = table_scan.DaskTableScanPlugin
 DaskFilterPlugin = filter.DaskFilterPlugin
@@ -13,6 +13,8 @@ DaskLimitPlugin = limit.DaskLimitPlugin
 SubqueryAlias = subquery_alias.SubqueryAlias
 ExplainPlugin = explain.ExplainPlugin
 DaskEmptyRelationPlugin = empty.DaskEmptyRelationPlugin
+DaskWindowPlugin = window.DaskWindowPlugin
 
 ALL_PLUGINS = (DaskTableScanPlugin, DaskFilterPlugin, DaskProjectPlugin, DaskJoinPlugin, DaskCrossJoinPlugin,
-               DaskAggregatePlugin, DaskSortPlugin, DaskLimitPlugin, SubqueryAlias, ExplainPlugin, DaskEmptyRelationPlugin)
+               DaskAggregatePlugin, DaskSortPlugin, DaskLimitPlugin, SubqueryAlias, ExplainPlugin, DaskEmptyRelationPlugin,
+               DaskWindowPlugin)

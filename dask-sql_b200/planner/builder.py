@@ -94,6 +94,8 @@ class Binder:
             pred = self.bind_expr(q.where, plan.schema)
             if pred.contains_agg():
                 self.err("Aggregate functions are not allowed in WHERE")
+            if pred.contains_window():
+                self.err("Window functions are not allowed in WHERE")
             plan = P.Filter(plan, pred)
 
         # select list
@@ -108,9 +110,14 @@ class Binder:
             else:
                 items.append((self.bind_expr(e, plan.schema), alias))
         aliases = {a: e for e, a in items if a}
+        # window calls of ORDER BY, bound where the SELECT list's are (they may read aggregates too)
+        order_windows = {j: self.bind_expr(e, plan.schema) for j, (e, _, _) in enumerate(q.order_by or [])
+                         if e.kind == "window"}
         having = self.bind_expr(q.having, plan.schema, aliases) if q.having is not None else None
+        if having is not None and having.contains_window():
+            self.err("Window functions are not allowed in HAVING")
         is_agg = bool(q.group_by) or any(e.contains_agg() for e, _ in items) or \
-            (having is not None and having.contains_agg())
+            (having is not None and having.contains_agg()) or any(w.contains_agg() for w in order_windows.values())
 
         if is_agg:
             group_exprs = []
@@ -124,6 +131,8 @@ class Binder:
                     group_exprs.append(aliases[g.parts[0]])
                 else:
                     group_exprs.append(self.bind_expr(g, plan.schema))
+            if any(g.contains_window() for g in group_exprs):
+                self.err("Window functions are not allowed in GROUP BY")
             agg_calls: List[PyExpr] = []
 
             def collect(e: PyExpr):
@@ -131,13 +140,15 @@ class Binder:
                     if not any(a.display() == e.display() for a in agg_calls):
                         agg_calls.append(e)
                     return
-                for c in e.args:
+                for c in (e.window_exprs() if e.kind == "window" else e.args):
                     collect(c)
 
             for e, _ in items:
                 collect(e)
             if having is not None:
                 collect(having)
+            for w in order_windows.values():
+                collect(w)
             agg_plan = P.Aggregate(plan, group_exprs, agg_calls)
 
             def rewrite(e: PyExpr) -> PyExpr:
@@ -152,22 +163,58 @@ class Binder:
                              "aggregate function")
                 out = e.clone()
                 out.args = [rewrite(a) for a in e.args]
+                if e.kind == "window":
+                    out.partition = [rewrite(x) for x in e.partition]
+                    out.order = [(rewrite(x), a, nf) for x, a, nf in e.order]
                 return out
 
             plan = agg_plan
             if having is not None:
                 plan = P.Filter(plan, rewrite(having))
-            proj = []
-            for e, alias in items:
-                r = rewrite(e)
-                name = alias if alias else None
-                if name is None and e.kind != "column":
-                    name = None  # display name of the aggregate output column
-                proj.append(PyExpr("alias", r.sql_type, name=name, args=[r]) if name else r)
-            plan = P.Projection(plan, proj)
-        else:
-            proj = [PyExpr("alias", e.sql_type, name=a, args=[e]) if a else e for e, a in items]
-            plan = P.Projection(plan, proj)
+            items = [(rewrite(e), alias) for e, alias in items]
+            order_windows = {j: rewrite(w) for j, w in order_windows.items()}
+
+        # window calls: computed by a Window node between the rows they read and the projection
+        windows: List[PyExpr] = []
+
+        def collect_windows(e: PyExpr):
+            if e.kind == "window":
+                if not any(w.display() == e.display() for w in windows):
+                    windows.append(e)
+                return
+            for c in e.children():
+                collect_windows(c)
+
+        def window_columns(e: PyExpr) -> PyExpr:
+            if e.kind == "window":
+                return P.col(None, e.display(), e.sql_type)
+            out = e.clone()
+            out.args = [window_columns(a) for a in e.args]
+            return out
+
+        for e, _ in items:
+            collect_windows(e)
+        for w in order_windows.values():
+            collect_windows(w)
+        if windows:
+            plan = P.Window(plan, windows)
+            items = [(window_columns(e), a) for e, a in items]
+        proj = [PyExpr("alias", e.sql_type, name=a, args=[e]) if a else e for e, a in items]
+        # an ORDER BY window call that the SELECT list does not output rides along as a hidden column, dropped
+        # again after the sort
+        def passes(e):       # the Window column a projection item outputs unchanged, or None
+            inner = e.args[0] if e.kind == "alias" else e
+            return inner.name if inner.kind == "column" and inner.qualifier is None else None
+
+        hidden = []
+        for w in order_windows.values():
+            if all(passes(e) != w.display() for e in proj + hidden):
+                hidden.append(P.col(None, w.display(), w.sql_type))
+        if hidden and q.distinct:
+            raise NotImplementedError("with SELECT DISTINCT, a window function in ORDER BY must also be in the "
+                                      "SELECT list")
+        plan = P.Projection(plan, proj + hidden)
+        visible = plan.schema[:len(proj)]
 
         if q.distinct:
             plan = P.Distinct(plan)
@@ -177,6 +224,11 @@ class Binder:
                 if e.kind == "lit" and isinstance(e.value, int) and not isinstance(e.value, bool):
                     f = plan.schema[e.value - 1]
                     b = P.col(f.qualifier, f.getName(), f.sql_type)
+                elif e.kind == "window":
+                    # by the Window node's output column, which the projection passes on
+                    w = order_windows[len(keys)]
+                    f = plan.schema[next(i for i, x in enumerate(proj + hidden) if passes(x) == w.display())]
+                    b = P.col(f.qualifier, f.getName(), f.sql_type)
                 else:
                     b = self.bind_expr(e, plan.schema, order_by_fallback=items)
                 keys.append((b, asc, (not asc) if nulls_first is None else nulls_first))
@@ -185,6 +237,8 @@ class Binder:
             fetch = q.limit.value if q.limit is not None else None
             skip = q.offset.value if q.offset is not None else 0
             plan = P.Limit(plan, skip, fetch)
+        if hidden:
+            plan = P.Projection(plan, [P.col(f.qualifier, f.getName(), f.sql_type) for f in visible])
         return plan
 
     def _empty_relation(self):
@@ -346,8 +400,12 @@ class Binder:
                 ty = _arith_type(ty, t.sql_type) if t.sql_type in _NUMERIC + ("NULL",) and ty in _NUMERIC + ("NULL",) \
                     else t.sql_type
             return PyExpr("case", ty, args=args)
+        if k == "window":
+            return self._bind_window(e, rec)
         if k == "func":
             name = e.name
+            if name in _WINDOW_ONLY:
+                raise NotImplementedError(f"{name} is a window function: it needs an OVER (...) clause")
             if name in P.AGG_FUNCS:
                 name = "AVG" if name == "MEAN" else name
                 args = [] if e.star else [rec(a) for a in e.args]
@@ -360,6 +418,8 @@ class Binder:
                     self.err(f"{name} takes exactly one argument")
                 if any(a.contains_agg() for a in args):
                     self.err("Aggregate function calls cannot be nested")
+                if any(a.contains_window() for a in args):
+                    self.err(f"A window function cannot be the argument of the aggregate {name}")
                 if name not in ("COUNT", "MIN", "MAX") and any(a.sql_type == "VARCHAR" for a in args):
                     raise NotImplementedError(f"{name} of a VARCHAR: only COUNT, MIN and MAX aggregate strings")
                 if name not in ("COUNT", "MIN", "MAX") and any(a.sql_type in _TEMPORAL for a in args):
@@ -378,6 +438,8 @@ class Binder:
                 else:
                     ty = args[0].sql_type
                 filt = rec(e.filter) if e.filter is not None else None
+                if filt is not None and filt.contains_window():
+                    self.err(f"A window function cannot be in the FILTER clause of the aggregate {name}")
                 return PyExpr("agg", ty, name=name, args=args, distinct=e.distinct, filter=filt)
             if name in _TEMPORAL_FUNCS:
                 return self._bind_temporal(name, e.args, rec)
@@ -390,6 +452,72 @@ class Binder:
                 return self._bind_math(name, args)
             self.err(f"Function {name} is outside the int64/float64 hot path of this layer")
         self.err(f"Unsupported expression {k}")
+
+    # -- window calls ---------------------------------------------------------------------------
+    def _bind_window(self, node, rec) -> PyExpr:
+        """f(args) OVER (PARTITION BY ... ORDER BY ... frame): frame -> (is_range, lo, hi), offsets from the row,
+        -inf / +inf for UNBOUNDED.  Without ORDER BY the default frame is the whole partition; with it, RANGE
+        BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW (through the row's last peer)."""
+        f = node.func
+        name = "AVG" if f.name == "MEAN" else f.name
+        if name in _WINDOW_REFUSED:
+            raise NotImplementedError(f"{name} is not supported as a window function; the window functions are "
+                                      f"{', '.join(P.WINDOW_FUNCS)}")
+        if name not in P.WINDOW_FUNCS:
+            if name in P.AGG_FUNCS:
+                raise NotImplementedError(f"{name} OVER (...) is not supported; the window aggregates are COUNT, SUM, "
+                                          "AVG, MIN and MAX")
+            self.err(f"{name} is not a window function")
+        if f.distinct:
+            raise NotImplementedError(f"{name}(DISTINCT ...) OVER (...) is not supported")
+        if f.filter is not None:
+            raise NotImplementedError(f"{name}(...) FILTER (WHERE ...) OVER (...) is not supported")
+        args = [] if f.star else [rec(a) for a in f.args]
+        if any(a.contains_window() for a in args):
+            self.err("Window function calls cannot be nested")
+        if name in ("ROW_NUMBER", "RANK", "DENSE_RANK"):
+            if args or f.star:
+                self.err(f"{name} takes no arguments")
+        elif name == "COUNT":
+            if len(args) > 1:
+                self.err("COUNT takes one argument or *")
+        elif len(args) != 1:
+            self.err(f"{name} takes exactly one argument")
+        if name in ("SUM", "AVG") and (args[0].sql_type == "VARCHAR" or args[0].sql_type in _TEMPORAL):
+            raise NotImplementedError(f"{name} of a {args[0].sql_type}: only COUNT, MIN, MAX, FIRST_VALUE and "
+                                      "LAST_VALUE take strings, dates and timestamps")
+        if name in ("ROW_NUMBER", "RANK", "DENSE_RANK", "COUNT"):
+            ty = "BIGINT"
+        elif name == "AVG":
+            ty = "DOUBLE"
+        elif name == "SUM":
+            ty = _norm_type(args[0].sql_type) if args[0].sql_type != "BOOLEAN" else "BIGINT"
+        else:
+            ty = args[0].sql_type
+        partition = [rec(p) for p in node.partition]
+        order = [(rec(x), asc, (not asc) if nf is None else nf) for x, asc, nf in node.order]
+        if any(x.contains_window() for x in partition + [o for o, _, _ in order]):
+            self.err("Window function calls cannot be nested")
+        inf = float("inf")
+        if node.frame is None:
+            frame = (True, -inf, 0) if order else (False, -inf, inf)
+        else:
+            fr = node.frame
+
+            def bound(b):
+                kind, v = b
+                return v * inf if kind == "unbounded" else v
+
+            if fr.unit == "RANGE" and "offset" in (fr.lo[0], fr.hi[0]):
+                raise NotImplementedError("RANGE frames with an offset (n PRECEDING / FOLLOWING) are not supported; "
+                                          "use ROWS, or RANGE with UNBOUNDED and CURRENT ROW bounds")
+            lo, hi = bound(fr.lo), bound(fr.hi)
+            if lo == inf:
+                self.err("A window frame cannot start at UNBOUNDED FOLLOWING")
+            if hi == -inf:
+                self.err("A window frame cannot end at UNBOUNDED PRECEDING")
+            frame = (fr.unit == "RANGE", lo, hi)
+        return PyExpr("window", ty, name=name, args=args, partition=partition, order=order, frame=frame)
 
     # -- RAND / RANDOM / RAND_INTEGER and TABLESAMPLE ------------------------------------------
     @staticmethod
@@ -534,6 +662,8 @@ class Binder:
 
 
 _RAND_FUNCS = ("RAND", "RANDOM", "RAND_INTEGER")
+_WINDOW_REFUSED = ("LAG", "LEAD", "NTILE", "NTH_VALUE", "PERCENT_RANK", "CUME_DIST", "SINGLE_VALUE")
+_WINDOW_ONLY = ("ROW_NUMBER", "RANK", "DENSE_RANK", "FIRST_VALUE", "LAST_VALUE") + _WINDOW_REFUSED
 _TEMPORAL_FUNCS = ("EXTRACT", "DATE_PART", "DATEPART", "YEAR", "TIMESTAMPADD", "TIMESTAMPDIFF", "TIMESTAMPFLOOR",
                    "TIMESTAMPCEIL", "LAST_DAY")
 _MATH_UNARY = ("CEIL", "FLOOR", "TRUNCATE", "ROUND", "SIGN", "DEGREES", "RADIANS", "SQRT", "EXP", "LN", "LOG10", "CBRT",

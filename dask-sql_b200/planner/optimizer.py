@@ -151,7 +151,8 @@ def push_filters(plan: P.LogicalPlan, preds: List[PyExpr]) -> P.LogicalPlan:
         new = P.Aggregate(push_filters(child, down), plan.group_exprs, plan.agg_exprs)
         return _wrap(new, keep)
 
-    # Distinct / Sort / Limit / CrossJoin / Explain: optimise below, keep predicates above
+    # Distinct / Sort / Limit / CrossJoin / Window / Explain: optimise below, keep predicates above (a filter
+    # below a Window would change the rows its functions see)
     plan.inputs = [push_filters(i, []) for i in plan.inputs]
     return _wrap(plan, preds)
 
@@ -207,6 +208,8 @@ def _refresh_schemas(plan: P.LogicalPlan):
         plan.schema = list(l.schema) + ([] if plan.how in ("LEFTSEMI", "LEFTANTI") else list(r.schema))
     elif isinstance(plan, P.CrossJoin):
         plan.schema = list(plan.inputs[0].schema) + list(plan.inputs[1].schema)
+    elif isinstance(plan, P.Window):
+        plan.schema = P.Window(plan.inputs[0], plan.window_exprs).schema
 
 
 def optimize(plan: P.LogicalPlan) -> P.LogicalPlan:

@@ -112,12 +112,15 @@ class PyExpr:
         self.negated = kw.get("negated", False)
         self.distinct = kw.get("distinct", False)
         self.filter: Optional["PyExpr"] = kw.get("filter")
+        self.partition: List["PyExpr"] = list(kw.get("partition", ()))
+        self.order = list(kw.get("order", ()))
+        self.frame = kw.get("frame")
         self.inputs: List["LogicalPlan"] = []   # plans whose concatenated schema getIndex() indexes
 
     # -- construction helpers
     def with_inputs(self, inputs):
         self.inputs = list(inputs)
-        for a in self.args:
+        for a in self.args + self.partition + [o for o, _, _ in self.order]:
             a.with_inputs(inputs)
         if self.filter is not None:
             self.filter.with_inputs(inputs)
@@ -135,14 +138,22 @@ class PyExpr:
         return out
 
     def contains_agg(self):
-        return self.kind == "agg" or any(c.contains_agg() for c in self.args)
+        return self.kind == "agg" or any(c.contains_agg() for c in
+                                         (self.window_exprs() if self.kind == "window" else self.args))
 
     def clone(self):
         e = PyExpr(self.kind, self.sql_type, qualifier=self.qualifier, name=self.name, value=self.value,
                    op=self.op, args=[a.clone() for a in self.args], negated=self.negated,
                    distinct=self.distinct, filter=self.filter.clone() if self.filter is not None else None)
         e.inputs = self.inputs
+        if self.kind == "window":
+            e.partition = [p.clone() for p in self.partition]
+            e.order = [(o.clone(), a, nf) for o, a, nf in self.order]
+            e.frame = self.frame
         return e
+
+    def contains_window(self):
+        return self.kind == "window" or any(c.contains_window() for c in self.children())
 
     # -- display (DataFusion-style names: they become output column names)
     def display(self) -> str:
@@ -205,9 +216,36 @@ class PyExpr:
             return self.args[0].display()
         if k == "scalarfn":
             return f"{self.name.lower()}({', '.join(a.display() for a in self.args)})"
+        if k == "window":
+            return f"{self.name}({'*' if self.name == 'COUNT' and not self.args else ', '.join(a.display() for a in self.args)}) {self.window_text()}"
         return k
 
     __repr__ = display
+
+    # window calls (kind == "window"): partition [PyExpr], order [(PyExpr, asc, nulls_first)],
+    # frame (is_range, lo, hi) with offsets from the row, -inf / +inf for UNBOUNDED
+    def spec_text(self) -> str:
+        parts = []
+        if self.partition:
+            parts.append(f"PARTITION BY [{', '.join(e.display() for e in self.partition)}]")
+        if self.order:
+            parts.append("ORDER BY [" + ", ".join(f"{e.display()} {'ASC' if a else 'DESC'} NULLS {'FIRST' if nf else 'LAST'}"
+                                                    for e, a, nf in self.order) + "]")
+        return " ".join(parts)
+
+    def window_text(self) -> str:
+        def bound(b):
+            if b == 0:
+                return "CURRENT ROW"
+            if b in (float("-inf"), float("inf")):
+                return f"UNBOUNDED {'PRECEDING' if b < 0 else 'FOLLOWING'}"
+            return f"{abs(b)} {'PRECEDING' if b < 0 else 'FOLLOWING'}"
+        is_range, lo, hi = self.frame
+        spec = self.spec_text()
+        return (spec + " " if spec else "") + f"{'RANGE' if is_range else 'ROWS'} BETWEEN {bound(lo)} AND {bound(hi)}"
+
+    def window_exprs(self):
+        return list(self.args) + list(self.partition or []) + [e for e, _, _ in self.order or []]
 
     def output_field(self) -> Tuple[Optional[str], str]:
         if self.kind == "column":
@@ -231,7 +269,8 @@ class PyExpr:
         return {"column": "Column", "literal": "Literal", "alias": "Alias", "agg": "AggregateFunction",
                 "binary": "BinaryExpr", "not": "Not", "isnull": "IsNull", "isnotnull": "IsNotNull",
                 "negative": "Negative", "between": "Between", "inlist": "InList", "cast": "Cast",
-                "case": "Case", "scalarfn": "ScalarFunction", "istrue": "IsTrue", "like": "Like"}[self.kind]
+                "case": "Case", "scalarfn": "ScalarFunction", "istrue": "IsTrue", "like": "Like",
+                "window": "WindowFunction"}[self.kind]
 
     def column_name(self, rel=None) -> str:
         return self.display()
@@ -619,6 +658,62 @@ class Aggregate(LogicalPlan):
     def describe(self):
         return (f"Aggregate: groupBy=[[{', '.join(e.display() for e in self.group_exprs)}]], "
                 f"aggr=[[{', '.join(e.display() for e in self.agg_exprs)}]]")
+
+
+WINDOW_FUNCS = ("ROW_NUMBER", "RANK", "DENSE_RANK", "COUNT", "SUM", "AVG", "MIN", "MAX", "FIRST_VALUE", "LAST_VALUE")
+
+
+class Window(LogicalPlan):
+    """Window calls over the input's rows: the input's fields, then one field per distinct call, named by its
+    display (src/sql/logical/window.rs).  getGroups() lists the distinct (PARTITION BY, ORDER BY) specs, each
+    with its calls; calls of one spec share its sort."""
+    node_type = "Window"
+
+    def __init__(self, child, window_exprs: Sequence[PyExpr]):
+        super().__init__([child])
+        self.window_exprs = list(window_exprs)
+        self.schema = list(child.schema)
+        for e in self.window_exprs:
+            self.schema.append(RelDataTypeField(None, e.display(), e.sql_type, len(self.schema)))
+
+    def window(self):
+        return self
+
+    def getGroups(self):
+        """[(spec text, [window call])] in order of first appearance"""
+        groups = {}
+        for e in self.window_exprs:
+            groups.setdefault(e.spec_text(), []).append(e)
+        return list(groups.items())
+
+    def getPartitionExprs(self, e: PyExpr):
+        return list(e.partition)
+
+    def getSortExprs(self, e: PyExpr):
+        out = []
+        for x, asc, nulls_first in e.order:
+            s = PyExpr("sort", x.sql_type, args=[x]).with_inputs(self.inputs)
+            s.ascending, s.nulls_first = asc, nulls_first
+            out.append(s)
+        return out
+
+    def getWindowFuncName(self, e: PyExpr):
+        return e.name
+
+    def getArgs(self, e: PyExpr):
+        return list(e.args)
+
+    def getWindowFrame(self, e: PyExpr):
+        return e.frame
+
+    def expressions(self):
+        return [x for e in self.window_exprs for x in e.window_exprs()]
+
+    def describe(self):
+        lines = []
+        for spec, calls in self.getGroups():
+            lines.append(f"[{spec or 'whole input'}]: " + ", ".join(c.display() for c in calls))
+        return "Window: " + "; ".join(lines)
 
 
 class Distinct(LogicalPlan):

@@ -14,7 +14,9 @@ Expressions: literals (incl. DATE '...', TIMESTAMP '...', INTERVAL '...' [unit])
 + - * / %, comparisons, AND OR NOT, IS [NOT] NULL, [NOT] BETWEEN, [NOT] IN (list), CAST(e AS type),
 e [NOT] LIKE | ILIKE 'pattern' [ESCAPE 'c'],
 CASE WHEN, EXTRACT(field FROM e), FLOOR / CEIL(e TO unit), function calls incl. aggregates with
-DISTINCT and FILTER (WHERE ...).
+DISTINCT and FILTER (WHERE ...), and window calls  f(...) OVER ([PARTITION BY e, ...] [ORDER BY ...] [frame])
+with frame := ROWS | RANGE  BETWEEN bound AND bound | bound,
+     bound := UNBOUNDED PRECEDING | n PRECEDING | CURRENT ROW | n FOLLOWING | UNBOUNDED FOLLOWING.
 
 Statements around the path (custom statements of the reference's parser, src/parser.rs):
   CREATE [OR REPLACE] TABLE|VIEW [IF NOT EXISTS] [schema.]name AS [(] query [)]
@@ -22,7 +24,8 @@ Statements around the path (custom statements of the reference's parser, src/par
   DROP TABLE [IF EXISTS] [schema.]name
   ANALYZE TABLE [schema.]name COMPUTE STATISTICS FOR ALL COLUMNS | COLUMNS c1 [, c2 ...]
 CREATE / DROP / TABLE / VIEW / IF / EXISTS / REPLACE / ANALYZE / COMPUTE / STATISTICS / FOR / COLUMNS and
-TABLESAMPLE / BERNOULLI / SYSTEM / REPEATABLE are contextual words, not reserved.
+TABLESAMPLE / BERNOULLI / SYSTEM / REPEATABLE, and OVER / PARTITION / ROWS / RANGE / UNBOUNDED / PRECEDING /
+FOLLOWING / CURRENT / ROW are contextual words, not reserved.
 
 Every RAND / RANDOM / RAND_INTEGER call and every TABLESAMPLE clause gets its call-site number `site`
 (1, 2, 3 ... in textual order), which keys its random numbers apart from the statement's other ones.
@@ -284,24 +287,10 @@ class Parser:
             while self.eat_op(","):
                 group_by.append(self.parse_expr())
         having = self.parse_expr() if self.eat_kw("HAVING") else None
-        order_by = []
-        if self.eat_kw("ORDER"):
-            self.expect_kw("BY")
-            while True:
-                e = self.parse_expr()
-                asc = True
-                if self.eat_kw("DESC"):
-                    asc = False
-                else:
-                    self.eat_kw("ASC")
-                nulls_first = None
-                if self.eat_kw("NULLS"):
-                    nulls_first = bool(self.eat_kw("FIRST"))
-                    if not nulls_first:
-                        self.expect_kw("LAST")
-                order_by.append((e, asc, nulls_first))
-                if not self.eat_op(","):
-                    break
+        if self.at_window_clause():
+            raise NotImplementedError("the WINDOW clause (named windows) is not supported; write the window "
+                                      "specification inline in OVER (...)")
+        order_by = self.parse_order_items() if self.eat_kw("ORDER") else []
         limit = offset = None
         if self.eat_kw("LIMIT"):
             limit = self.parse_expr()
@@ -382,9 +371,13 @@ class Parser:
         alias = None
         if self.eat_kw("AS"):
             alias = self.ident()
-        elif self.cur.kind == "id" and not self.at_tablesample():
+        elif self.cur.kind == "id" and not self.at_tablesample() and not self.at_window_clause():
             alias = self.ident()
         return Node("table", name=parts, alias=alias, sample=self.parse_tablesample())
+
+    def at_window_clause(self):
+        """WINDOW name AS (...)"""
+        return self.at_word("WINDOW") and self.toks[self.i + 1].kind == "id" and self.toks[self.i + 2].val == "AS"
 
     def at_tablesample(self):
         if not self.at_word("TABLESAMPLE"):
@@ -409,6 +402,79 @@ class Parser:
             seed = self.parse_expr()
             self.expect_op(")")
         return Node("tablesample", method=method, p=p, seed=seed, site=site)
+
+    # -- window functions
+    def parse_over(self, call: Node) -> Node:
+        """call OVER ([PARTITION BY e, ...] [ORDER BY e [ASC|DESC] [NULLS FIRST|LAST], ...] [frame])"""
+        self.expect_word("OVER")
+        if not self.at_op("("):
+            raise NotImplementedError("a named window (OVER name / the WINDOW clause) is not supported; write the "
+                                      "window specification inline")
+        self.i += 1
+        partition = []
+        if self.eat_word("PARTITION"):
+            self.expect_kw("BY")
+            partition.append(self.parse_expr())
+            while self.eat_op(","):
+                partition.append(self.parse_expr())
+        order = self.parse_order_items() if self.eat_kw("ORDER") else []
+        frame = None
+        if self.at_word("ROWS", "RANGE", "GROUPS"):
+            frame = self.parse_frame()
+        self.expect_op(")")
+        return Node("window", func=call, partition=partition, order=order, frame=frame)
+
+    def parse_frame(self) -> Node:
+        unit = self.eat_word("ROWS", "RANGE", "GROUPS")
+        if unit == "GROUPS":
+            raise NotImplementedError("GROUPS window frames are not supported; use ROWS or RANGE")
+        if self.eat_kw("BETWEEN"):
+            lo = self.parse_frame_bound()
+            self.expect_kw("AND")
+            hi = self.parse_frame_bound()
+        else:
+            lo, hi = self.parse_frame_bound(), ("current", 0)
+        if self.at_word("EXCLUDE"):
+            raise NotImplementedError("EXCLUDE in a window frame is not supported")
+        return Node("frame", unit=unit, lo=lo, hi=hi)
+
+    def parse_frame_bound(self):
+        """-> (kind, n): ("unbounded", -1 | +1), ("current", 0), ("offset", -n | +n)"""
+        if self.eat_word("UNBOUNDED"):
+            which = self.eat_word("PRECEDING", "FOLLOWING")
+            if which is None:
+                self.error("Expected PRECEDING or FOLLOWING")
+            return ("unbounded", -1 if which == "PRECEDING" else 1)
+        if self.eat_word("CURRENT"):
+            self.expect_word("ROW")
+            return ("current", 0)
+        if self.cur.kind != "num" or not re.fullmatch(r"\d+", self.cur.val):
+            self.error("A window frame offset is a non-negative integer literal")
+        k = int(self.cur.val)
+        self.i += 1
+        which = self.eat_word("PRECEDING", "FOLLOWING")
+        if which is None:
+            self.error("Expected PRECEDING or FOLLOWING")
+        return ("offset", -k if which == "PRECEDING" else k)
+
+    def parse_order_items(self):
+        self.expect_kw("BY")
+        out = []
+        while True:
+            e = self.parse_expr()
+            asc = True
+            if self.eat_kw("DESC"):
+                asc = False
+            else:
+                self.eat_kw("ASC")
+            nulls_first = None
+            if self.eat_kw("NULLS"):
+                nulls_first = bool(self.eat_kw("FIRST"))
+                if not nulls_first:
+                    self.expect_kw("LAST")
+            out.append((e, asc, nulls_first))
+            if not self.eat_op(","):
+                return out
 
     # -- expressions (precedence climbing)
     def parse_expr(self) -> Node:
@@ -618,7 +684,10 @@ class Parser:
                     self.expect_kw("WHERE")
                     filt = self.parse_expr()
                     self.expect_op(")")
-                return Node("func", name=name.upper(), args=args, distinct=distinct, star=star, filter=filt)
+                call = Node("func", name=name.upper(), args=args, distinct=distinct, star=star, filter=filt)
+                if self.at_word("OVER"):
+                    return self.parse_over(call)
+                return call
             parts = [name]
             while self.eat_op("."):
                 parts.append(self.ident())

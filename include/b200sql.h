@@ -625,6 +625,91 @@ typedef struct b2_select {
 int32_t b2_select_hist(const b2_col_t* col, int64_t n, const b2_select_t* sel, uint64_t* hist, int64_t* out,
                        uint64_t* out_count, void* stream);
 
+/* ---- window functions: f(...) OVER (PARTITION BY ... ORDER BY ... frame) ---------------------- */
+/* Every array below is indexed by the sorted position i < n, the order b2_sort_by left in idx (partition
+ * keys, then order keys).  Replaces physical/rel/logical/window.py's groupby().rolling / expanding.
+ *
+ * flags[i] (uint8, zeroed by the caller): bit 0 = i starts a partition, bit 1 = i starts a peer group.
+ * b2_window_heads ORs in the bits of one key column: position 0, and every position whose key image
+ * (b2_sort_by's: NULL and NaN alike, -0.0 == +0.0) differs from position i-1's, gets bits 0|1 when
+ * partition != 0 (a PARTITION BY key), bit 1 otherwise (an ORDER BY key).  Call once per key. */
+int32_t b2_window_heads(const b2_col_t* key, const int32_t* idx, int64_t n, int32_t partition, uint8_t* flags,
+                        void* stream);
+/* Scratch of b2_window_positions / b2_window_scan for n positions. */
+int64_t b2_window_ws_bytes(int64_t n);
+/* ps[i] / qs[i]: first position of i's partition / peer group; dn[i]: DENSE_RANK (peer groups of the
+ * partition up to i).  pend[ps[i]] / qend[qs[i]]: last position of i's partition / peer group (written at
+ * the start positions only). */
+int32_t b2_window_positions(const uint8_t* flags, int64_t n, int32_t* ps, int32_t* qs, int32_t* dn, int32_t* pend,
+                            int32_t* qend, void* ws, void* stream);
+/* Segmented inclusive scans of a sorted argument column val (B2_I64, B2_F64 or B2_U8; NULL rows and NaN
+ * are skipped).  Segments start where flags & seg_mask (1: partitions, 2: peer groups); reverse != 0 runs
+ * from the end, so position i holds the scan of [i, end of its segment].
+ *   B2_WIN_SUM_I: val = int64 wrapping sum                     (int64[n])
+ *   B2_WIN_SUM_F: val / lo = double-double sum of the finite values (TwoSum / FastTwoSum), pinf / ninf =
+ *                 count of +inf / -inf                         (double[n] x 2, int32[n] x 2)
+ *   B2_WIN_MIN / B2_WIN_MAX: val = running min / max of the order image (int64 value; float64:
+ *                 b2_ordered_from_bits of its bits), INT64_MAX / INT64_MIN before the first value
+ * cnt (optional for every kind) = number of non-NULL values. */
+#define B2_WIN_SUM_I 0
+#define B2_WIN_SUM_F 1
+#define B2_WIN_MIN   2
+#define B2_WIN_MAX   3
+typedef struct b2_win_prefix {
+  void*    val;
+  double*  lo;
+  int32_t* cnt;
+  int32_t* pinf;
+  int32_t* ninf;
+} b2_win_prefix_t;
+int32_t b2_window_scan(const uint8_t* flags, const b2_col_t* val, int64_t n, int32_t kind, int32_t seg_mask,
+                       int32_t reverse, const b2_win_prefix_t* out, void* ws, void* stream);
+/* Sparse table for MIN / MAX over frames of bounded width: table[k * n + i] = min / max (is_max) of the
+ * order images of positions [i, i + 2^k), NULL = the identity, k < levels (levels >= 1). */
+int32_t b2_window_rmq(const b2_col_t* val, int64_t n, int32_t is_max, int32_t levels, int64_t* table,
+                      void* stream);
+/* One window function over every position.  The frame of position i is [lo, hi]: ROWS bounds are offsets
+ * from i (-k: k PRECEDING, 0: CURRENT ROW, +k: k FOLLOWING, -/+B2_WIN_UNBOUNDED); RANGE (range != 0) takes
+ * only -B2_WIN_UNBOUNDED / 0 / +B2_WIN_UNBOUNDED, CURRENT ROW meaning i's first / last peer.  The frame is
+ * clamped to the partition; it may be empty.  Results, per fn:
+ *   ROW_NUMBER, RANK, DENSE_RANK, COUNT_STAR, COUNT: int64, never NULL (frame ignored by the first three)
+ *   SUM_I: int64 (pre from B2_WIN_SUM_I); SUM_F, AVG: double (pre from B2_WIN_SUM_F; AVG's cnt too)
+ *   MIN / MAX: val's dtype (B2_U8 -> int64).  pre: forward partition scan, used when lo is the partition
+ *     start; suf: reverse partition scan, when hi is its end; peer: forward peer-group scan, for RANGE
+ *     CURRENT ROW .. CURRENT ROW; rmq (rmq_levels levels), otherwise.  Each needs cnt.
+ *   FIRST_VALUE / LAST_VALUE: val at lo / hi, in val's dtype.
+ * SUM, AVG, MIN, MAX, FIRST_VALUE and LAST_VALUE are NULL for an empty frame, SUM to MAX also when the frame
+ * holds no non-NULL value.  out_valid: a bitmap of (n + 31) / 32 words, written whole (NULL: not wanted,
+ * allowed for the never-NULL functions). */
+#define B2_WIN_UNBOUNDED ((int64_t)1 << 40)
+#define B2_WF_ROW_NUMBER  0
+#define B2_WF_RANK        1
+#define B2_WF_DENSE_RANK  2
+#define B2_WF_COUNT_STAR  3
+#define B2_WF_COUNT       4
+#define B2_WF_SUM_I       5
+#define B2_WF_SUM_F       6
+#define B2_WF_AVG         7
+#define B2_WF_MIN         8
+#define B2_WF_MAX         9
+#define B2_WF_FIRST_VALUE 10
+#define B2_WF_LAST_VALUE  11
+typedef struct b2_win_frame {
+  int32_t fn, range;
+  int64_t lo, hi, n;
+  const int32_t *ps, *qs, *dn, *pend, *qend;
+  b2_col_t val;
+  b2_win_prefix_t pre, suf, peer;
+  const int64_t* rmq;
+  int32_t rmq_levels, pad_;
+  void* out;
+  uint32_t* out_valid;
+} b2_win_frame_t;
+int32_t b2_window_frame(const b2_win_frame_t* f, void* stream);
+/* inv[idx[i]] = i: the positions of the input rows, so that b2_gather(result, inv) returns a window
+ * result in input row order. */
+int32_t b2_window_invert(const int32_t* idx, int64_t n, int32_t* inv, void* stream);
+
 /* ---- fused filter -> join -> group-by (star pipeline) ----------------------------- */
 /* out_slot[i] = key[i]-kmin (NULL key -> null_slot) as int32: turns a dense group-key column of
  * the build side into group-table slot numbers. */

@@ -20,6 +20,11 @@ WANT = {
     "groupby_dense_hh": r"b2_groupby_dense_hh_kernel",
     "groupby_dense_grouped": r"b2_groupby_dense_grouped_kernel",
     "scan_agg": r"b2_scan_agg_kernelILb0E",
+    "window_heads": r"b2_window_heads_kernel",
+    "window_rescan_sumf": r"b2_window_rescan_kernelI14b2_win_sumf_op",
+    "window_rescan_pos": r"b2_window_rescan_kernelI13b2_win_pos_op",
+    "window_rmq_level": r"b2_window_rmq_level_kernel",
+    "window_frame": r"b2_window_frame_kernel",
 }
 INTERESTING = re.compile(r"\b(LDG|STG|REDG|ATOMG|ATOMS|ATOM|RED|LDS|STS|MATCH|VOTE|SHFL|REDUX|UBLKCP|SYNCS|BAR|CCTL|LDGSTS|UTMALDG|LD|ST|NANOSLEEP|MEMBAR|ERRBAR)\b")
 
