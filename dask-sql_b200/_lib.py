@@ -75,6 +75,14 @@ class JoinTable(C.Structure):
                 ("range", C.c_int64)]
 
 
+MARK_MAX_TERMS = 4
+MARK_NULL_AWARE, MARK_BUILD_NONEMPTY, MARK_BUILD_HAS_NULL, MARK_WHERE = 1, 2, 4, 8
+
+
+class MarkTerm(C.Structure):
+    _fields_ = [("probe_col", C.c_int32), ("build", Col), ("cmp", C.c_int32)]
+
+
 JA_P, JA_B, JA_MUL, JA_ADD, JA_SUB, JA_RSUB, JA_ROWS = range(7)
 JA_MAX_BUILD = 4
 
@@ -134,6 +142,7 @@ class PeerMerge(C.Structure):
 
 assert C.sizeof(Col) == 24 and C.sizeof(Term) == 32 and C.sizeof(Scan) == 656
 assert C.sizeof(AggState) == 152 and C.sizeof(Instr) == 24 and C.sizeof(Prog) == 1544
+assert C.sizeof(MarkTerm) == 40
 assert C.sizeof(JoinTable) == 152 and C.sizeof(StarLookup) == 64 and C.sizeof(PeerMerge) == 544
 assert C.sizeof(Select) == 80
 
@@ -215,6 +224,8 @@ _SIGS = {
     "b2_join_onepass": [C.POINTER(Scan), C.POINTER(C.c_int32), C.POINTER(JoinTable), C.c_int32, _P, C.c_int32,
                         C.POINTER(C.c_int32), C.POINTER(_P), C.POINTER(_P), C.c_int32, C.POINTER(Col),
                         C.POINTER(C.c_int64), C.POINTER(_P), C.POINTER(_P), _P],
+    "b2_join_mark": [C.POINTER(Scan), C.POINTER(C.c_int32), C.POINTER(JoinTable), C.POINTER(MarkTerm), C.c_int32,
+                     C.c_int32, _P, _P, _P],
     "b2_join_agg": [C.POINTER(Scan), C.c_int32, C.POINTER(JoinTable), C.c_int32, C.POINTER(Col), C.POINTER(C.c_int64),
                     C.POINTER(JoinAgg), C.c_int32, _P, _P, C.c_int32, _P, _P],
     "b2_range_partition_hist": [C.POINTER(Scan), C.c_int32, C.c_int64, C.c_int64, C.c_int32, C.c_int32, _P, _P],
@@ -327,6 +338,7 @@ join_write_gather_keyed = _wrap("b2_join_write_gather_keyed")
 join_key_layout = _wrap("b2_join_key_layout")
 join_onepass = _wrap("b2_join_onepass")
 join_agg = _wrap("b2_join_agg")
+join_mark = _wrap("b2_join_mark")
 range_partition = _wrap("b2_range_partition")
 range_partition_hist = _wrap("b2_range_partition_hist")
 range_partition_scan = _wrap("b2_range_partition_scan")

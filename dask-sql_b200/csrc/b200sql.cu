@@ -36,6 +36,7 @@ int b2_sm_count() {
 #include "filter.cuh"
 #include "groupby.cuh"
 #include "join.cuh"
+#include "mark.cuh"
 #include "joinagg.cuh"
 #include "sort.cuh"
 #include "window.cuh"

@@ -731,3 +731,17 @@ def join_probe(scan, probe_keys, jt: JoinTable, mode, device, build_matched=None
         L.join_write(C.byref(scan), pk, C.byref(jt.struct), mode, ptr(tile_off), ptr(pidx), ptr(bidx),
                      ptr(build_matched), stream_ptr())
     return pidx, bidx, total
+
+
+def join_mark(scan, probe_keys, jt: JoinTable, terms, flags, device) -> DeviceColumn:
+    """The three-valued mark of an IN / EXISTS subquery over the rows of `scan` (b2_join_mark).
+    terms: [(probe slot, build DeviceColumn, B2 comparison)] -> a B2_U8 column with validity."""
+    n = scan.n
+    out = torch.empty(max(n, 1), dtype=torch.uint8, device=device)[:n]
+    valid = torch.empty(bitmap_words(n), dtype=torch.int32, device=device)
+    pk = (C.c_int32 * len(probe_keys))(*probe_keys)
+    mt = (L.MarkTerm * max(1, len(terms)))()
+    for i, (slot, col, cmp) in enumerate(terms):
+        mt[i].probe_col, mt[i].build, mt[i].cmp = slot, col.as_struct(), cmp
+    L.join_mark(C.byref(scan), pk, C.byref(jt.struct), mt, len(terms), flags, ptr(out), ptr(valid), stream_ptr())
+    return DeviceColumn(out, valid, U8)

@@ -26,10 +26,11 @@ from . import expr as E
 from . import parallel as P
 from . import rand as R
 from . import strings as S
+from . import temporal as T
 from .device import DeviceColumn, TermSpec, I64, F64, U8
 from .expr import Expr, ColRef, Lit, Call
 from .frame import (LazyFrame, Source, TableSource, JoinSource, AggSource, SortSource, LimitSource, WindowSource,
-                    SAMPLE_MASK)
+                    MarkSource, SAMPLE_MASK)
 from .table import DeviceTable, HostColumn
 
 DENSE_MAX_SLOTS = 1 << 27          # direct-address group tables up to 128M slots
@@ -37,7 +38,7 @@ _TORCH_DT = {I64: torch.int64, F64: torch.float64, U8: torch.uint8}
 
 # counters the bench / tests read to prove which kernels ran
 stats = {"launches": 0, "star_fused": 0, "dense_groupby": 0, "hash_groupby": 0, "dense_join": 0,
-         "chain_join": 0, "keyed_join": 0, "partitioned_groupby": 0, "h2d_bytes": 0, "d2h_bytes": 0}
+         "chain_join": 0, "keyed_join": 0, "partitioned_groupby": 0, "h2d_bytes": 0, "d2h_bytes": 0, "marks": 0}
 
 
 # Optional per-launch timing of the dominant kernels (bench.py sets this to a list): each entry
@@ -621,6 +622,8 @@ def materialize(src: Source, needed: Set[str], top: bool = False, pred=None) -> 
         return [run_limit(src, needed)]
     if isinstance(src, WindowSource):
         return [run_window(src, needed)]
+    if isinstance(src, MarkSource):
+        return run_mark(src, needed)
     raise TypeError(f"unknown source {type(src).__name__}")
 
 
@@ -821,6 +824,84 @@ def run_window(src: WindowSource, needed: Set[str]) -> Part:
         for o, col in results:
             out[o] = D.gather(col, inv, False)
         _kernel_event_end(rec)
+    return out
+
+
+def mark_refusal(child: LazyFrame) -> Optional[str]:
+    """Why the rows of `child` cannot take a subquery mark here, or None."""
+    if P.world()[1] > 1 and frame_distribution(child) in ("sharded", "root"):
+        return ("IN / EXISTS subqueries over a sharded or root table on more than one GPU: each rank would mark "
+                "its rows against its own share of the subquery's rows")
+    return None
+
+
+_MARK_CMP = {"=": L.EQ, "!=": L.NE, "<": L.LT, "<=": L.LE, ">": L.GT, ">=": L.GE}
+
+
+def _mark_operands(a: Expr, b: Expr):
+    """one key or pair term, child side a and inner side b, on one comparable representation: VARCHAR keys
+    of two dictionaries translated (strings.join_keys), DATE / TIMESTAMP at the finer unit, booleans as int64,
+    and int64 beside float64 as float64 -- the rules of the join's keys (run_join, join.py's _same_unit_keys)"""
+    if E.is_varchar(a) or E.is_varchar(b):          # keys only: the binder refuses VARCHAR pair terms
+        a, b = S.join_keys(a, b, True)
+    ua, ub = T.unit_of(a.logical), T.unit_of(b.logical)
+    if ua is not None and ub is not None and ua != ub:
+        u = T.finer(ua, ub)
+        a, b = T.at_unit(a, u), T.at_unit(b, u)
+    if a.dtype == U8:
+        a = E.cast(a, I64)
+    if b.dtype == U8:
+        b = E.cast(b, I64)
+    if a.dtype != b.dtype:
+        a, b = E.cast(a, F64), E.cast(b, F64)
+    return a, b
+
+
+def run_mark(src: MarkSource, needed: Set[str]) -> List[Part]:
+    """The mark of an IN / EXISTS subquery over the child's rows, partition by partition: the subquery body is
+    materialised once, its key columns hashed by the join's build (D.JoinTable), and one b2_join_mark per child
+    partition walks each row's candidates and evaluates the pair terms."""
+    why = mark_refusal(src.child)
+    if why is not None:
+        raise NotImplementedError(why)
+    dev = _dev()
+    inputs = src.inputs()
+    names = [n for n in src.child.columns if n in needed or n in inputs]
+    parts = execute(src.child, names)
+    inner = src.inner
+    pk, bk = [], {}
+    for i, (c, b) in enumerate(src.keys):
+        a, bk[f"__bk{i}"] = _mark_operands(ColRef(c, *src.child.col_type(c)), inner.exprs[b])
+        pk.append(a)
+    pt = []
+    for t, (c, b, cmp, where) in enumerate(src.terms):
+        a, bk[f"__bt{t}"] = _mark_operands(ColRef(c, *src.child.col_type(c)), inner.exprs[b])
+        pt.append((a, _MARK_CMP[cmp] | (L.MARK_WHERE if where else 0)))
+    bpart = concat_parts(execute(LazyFrame(inner.source, bk, inner.pred)), list(bk))
+    jt = D.JoinTable([bpart[f"__bk{i}"] for i in range(len(pk))])
+    stats["launches"] += 1
+    flags = 0
+    if src.null_aware:
+        flags = L.MARK_NULL_AWARE
+        if bpart.n > 0:
+            flags |= L.MARK_BUILD_NONEMPTY
+            if bpart["__bk0"].ensure_stats().nulls > 0:
+                flags |= L.MARK_BUILD_HAS_NULL
+    out = []
+    for part in parts:
+        part = part.resolve()
+        ctx = ScanCtx(part, [])
+        kslots = [ctx.slot(e) for e in pk]
+        terms = [(ctx.slot(e), bpart[f"__bt{t}"], cmp) for t, (e, cmp) in enumerate(pt)]
+        stats["launches"] += 1
+        stats["marks"] += 1
+        rec = _kernel_event_begin("b2_join_mark", part.n)
+        mark = D.join_mark(ctx.scan(), kslots, jt, terms, flags, dev)
+        _kernel_event_end(rec)
+        res = Part({n: part[n] for n in names if n in needed}, part.n)
+        res.dist = part.dist
+        res[src.out] = mark
+        out.append(res)
     return out
 
 

@@ -152,6 +152,23 @@ class WindowSource(Source):
         return list(dict.fromkeys(out))
 
 
+class MarkSource(Source):
+    """The child's rows and columns plus `out`, the mark of an IN / EXISTS subquery (executor.run_mark): a
+    three-valued BOOLEAN per child row.  inner: the subquery body's frame; keys: [(child column, inner
+    column)] equality keys; terms: [(child column, inner column, cmp, where)] pair terms  child <cmp> inner;
+    null_aware: the one key is the operand of an uncorrelated IN."""
+
+    def __init__(self, child: "LazyFrame", inner: "LazyFrame", keys, terms, null_aware, out):
+        self.child, self.inner = child, inner
+        self.keys, self.terms, self.null_aware, self.out = list(keys), list(terms), null_aware, out
+        self.schema = OrderedDict((n, child.col_type(n)) for n in child.columns)
+        self.schema[out] = (U8, "bool")
+
+    def inputs(self):
+        """the child columns the mark reads"""
+        return list(dict.fromkeys([k for k, _ in self.keys] + [t[0] for t in self.terms]))
+
+
 class LimitSource(Source):
     """LIMIT / OFFSET over the child's row order."""
 

@@ -4,7 +4,9 @@ import logging
 import numpy as np
 
 from ....datacontainer import DataContainer
+from ....planner.plan import conjunction, conjuncts
 from ...rex import RexConverter
+from ...rex.core.subquery import attach_marks
 from ..base import BaseRelPlugin
 
 log = logging.getLogger(__name__)
@@ -31,6 +33,17 @@ class DaskFilterPlugin(BaseRelPlugin):
 
     def convert(self, rel, context) -> DataContainer:
         (child,) = self.assert_inputs(rel, 1, context)
-        keep = RexConverter.convert(rel, rel.filter().getCondition(), child, context=context)
+        cond = rel.filter().getCondition()
+        if cond.contains_subquery():
+            # the block's other conjuncts first, so that an IN / EXISTS mark is built over the rows they keep
+            plain = [c for c in conjuncts(cond) if not c.contains_subquery()]
+            if plain:
+                first = conjunction(plain).with_inputs(cond.inputs)
+                rest = conjunction([c for c in conjuncts(cond) if c.contains_subquery()]).with_inputs(cond.inputs)
+                keep = RexConverter.convert(rel, first, child, context=context)
+                child = DataContainer(filter_or_scalar(child.df, keep), child.column_container)
+                cond = rest
+            child = attach_marks(rel, [cond], child, context)
+        keep = RexConverter.convert(rel, cond, child, context=context)
         names = self.fix_column_to_row_type(child.column_container, rel.getRowType())
         return DataContainer(filter_or_scalar(child.df, keep), names)

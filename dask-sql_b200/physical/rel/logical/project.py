@@ -8,6 +8,7 @@ from ....datacontainer import DataContainer
 from ....planner import RexType
 from ....utils import new_temporary_column
 from ...rex import RexConverter
+from ...rex.core.subquery import attach_marks
 from ..base import BaseRelPlugin
 
 _REFERENCE = str(RexType.Reference)
@@ -18,6 +19,7 @@ class DaskProjectPlugin(BaseRelPlugin):
 
     def convert(self, rel, context) -> DataContainer:
         (child,) = self.assert_inputs(rel, 1, context)
+        child = attach_marks(rel, [expr for _, expr in rel.projection().getNamedProjects()], child, context)
         frame, names = child.df, child.column_container
         computed, backend_of = {}, {}
         for out_name, expr in rel.projection().getNamedProjects():

@@ -291,6 +291,7 @@ OPERATORS.update({
     "timestampceil": _temporal(lambda x, unit: T.floor_ceil(x, unit, True), 0),
     "last_day": _temporal(lambda x: T.add_months_expr(x, 0, to_last=True), 0),
 })
+
 # numeric functions (call.py:1091-1113, and SQRT)
 OPERATORS.update({name: _math(name) for name in ("ceil", "floor", "truncate", "round", "sign", "degrees", "radians",
                                                   "sqrt", "exp", "ln", "log10", "cbrt", "sin", "cos", "tan", "cot",
@@ -320,6 +321,9 @@ class RexCallPlugin(BaseRexPlugin):
         logger.debug("%s on %s", name, [str(LoggableDataFrame(o)) for o in operands])
         if name in ("rand", "rand_integer"):
             return _rand(name, operands, dc)
+        if name in ("in subquery", "exists"):       # call.py:996-1030; the mark column attach_marks added
+            from .subquery import mark_of
+            return mark_of(expr, dc)
         fn = OPERATORS.get(name)
         if fn is not None:
             return fn(operands, expr)

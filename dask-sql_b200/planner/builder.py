@@ -45,6 +45,15 @@ class Binder:
         self.sql, self.catalog, self.case_sensitive = sql, catalog, case_sensitive
         self._key = None          # the statement's key for RAND / TABLESAMPLE without a seed
         self.volatile = False     # the statement drew that key: re-planning it must draw a new one
+        # subqueries: the scope of the block enclosing the one being bound (None: a derived table, CTE, ON,
+        # GROUP BY ... where no correlation is allowed), the correlated conjuncts of each subquery's WHERE, and
+        # the common table expressions each block sees
+        self._outer: List[Optional[list]] = []
+        self._corr: List[list] = []
+        self._kind: List[str] = []          # "in" | "exists" | "scalar": the subquery each _corr entry is for
+        self._ctes: List[dict] = []
+        self._joins: List[list] = []        # per block: correlated scalar subqueries to LEFT JOIN onto its rows
+        self._nsq = 0
 
     def err(self, msg):
         raise ParsingException(self.sql, msg)
@@ -86,29 +95,114 @@ class Binder:
         return P.AnalyzeTable(schema_name, table_name.lower(), columns, columns or names)
 
     def bind_query(self, q: Node, ctes: Dict[str, P.LogicalPlan]) -> P.LogicalPlan:
-        ctes = dict(ctes)
-        for name, sub in q.ctes or []:
-            ctes[name] = self.bind_query(sub, ctes)
-        plan = self.bind_from(q.source, ctes) if q.source is not None else self._empty_relation()
+        # a subquery body binds its WHERE with the enclosing block's scope on top of self._outer; everything
+        # else of it, and any block it reads from, sees no outer scope
+        correlated = bool(self._outer) and self._outer[-1] is not None
+        self._outer.append(None)
+        try:
+            ctes = dict(ctes)
+            for name, sub in q.ctes or []:
+                ctes[name] = self.bind_query(sub, ctes)
+            plan = self.bind_from(q.source, ctes) if q.source is not None else self._empty_relation()
+        finally:
+            self._outer.pop()
+        self._ctes.append(ctes)
+        try:
+            return self._bind_block(q, plan, correlated)
+        finally:
+            self._ctes.pop()
+
+    def _bind_block(self, q: Node, plan: P.LogicalPlan, correlated: bool) -> P.LogicalPlan:
+        self._joins.append([])
+        try:
+            return self._bind_where(q, plan, correlated)
+        finally:
+            self._joins.pop()
+
+    def _apply_joins(self, plan: P.LogicalPlan) -> P.LogicalPlan:
+        """LEFT JOIN the grouped bodies of the correlated scalar subqueries bound so far onto `plan`"""
+        for alias, body, pairs in self._joins[-1]:
+            plan = P.Join(plan, P.SubqueryAlias(body, alias), "LEFT", pairs, None)
+        self._joins[-1].clear()
+        return plan
+
+    def _bind_where(self, q: Node, plan: P.LogicalPlan, correlated: bool) -> P.LogicalPlan:
+        corr = []
         if q.where is not None:
             pred = self.bind_expr(q.where, plan.schema)
             if pred.contains_agg():
                 self.err("Aggregate functions are not allowed in WHERE")
             if pred.contains_window():
                 self.err("Window functions are not allowed in WHERE")
-            plan = P.Filter(plan, pred)
+            if correlated:
+                local = []
+                for c in P.conjuncts(pred):
+                    (corr if _outer_columns(c) else local).append(c)
+                pred = P.conjunction(local)
+                corr = [self._split_correlated(c) for c in corr]
+            plan = self._apply_joins(plan)
+            if pred is not None:
+                plan = P.Filter(plan, pred)
+        self._outer.append(None)
+        try:
+            return self._bind_rest(q, plan, corr)
+        finally:
+            self._outer.pop()
+
+    def _split_correlated(self, c: PyExpr):
+        """a correlated conjunct -> (inner expression, op, outer expression): `inner op outer`"""
+        if c.kind == "binary" and c.op in _FLIP and not c.contains_subquery():
+            a, b = c.args
+            oa, ob = _outer_columns(a), _outer_columns(b)
+            ia, ib = len(a.columns()) > len(oa), len(b.columns()) > len(ob)
+            if ob and not oa and not ib:
+                return a, c.op, _strip_outer(b)
+            if oa and not ob and not ia:
+                return b, _FLIP[c.op], _strip_outer(a)
+        raise NotImplementedError(f"the correlated predicate {c.display()} must compare an expression of the "
+                                  "subquery's rows with an expression of the enclosing block's rows (= <> < <= > >=)")
+
+    def _bind_rest(self, q: Node, plan: P.LogicalPlan, corr) -> P.LogicalPlan:
 
         # select list
         items: List[Tuple[PyExpr, Optional[str]]] = []
         for e, alias in q["items"]:
             if e.kind == "star":
-                fields = [f for f in plan.schema if e.qualifier is None or f.qualifier == e.qualifier]
+                fields = [f for f in plan.schema if (e.qualifier is None or f.qualifier == e.qualifier) and
+                          not (f.qualifier or "").startswith(_SQ_ALIAS)]
                 if not fields:
                     self.err(f"Invalid qualifier {e.qualifier}")
                 for f in fields:
                     items.append((P.col(f.qualifier, f.getName(), f.sql_type), None))
             else:
                 items.append((self.bind_expr(e, plan.schema), alias))
+        plan = self._apply_joins(plan)
+        extra_groups = []
+        if corr:
+            # a correlated body outputs its select list, then the inner side of each correlated conjunct; a grouped
+            # body also groups by those (equality keys only), so each group lies within one correlation group
+            kind = self._kind[-1]
+            aggregated = any(e.contains_agg() for e, _ in items)
+            if kind == "scalar":
+                if q.group_by or q.having is not None or not aggregated or len(items) != 1:
+                    raise NotImplementedError("a correlated scalar subquery must be one aggregate over the correlated "
+                                              "rows, without GROUP BY or HAVING")
+                self._corr[-1].append(_count_kind(items[0][0]))
+                items[0] = (items[0][0], "__sv")
+            elif (q.group_by or q.having is not None or aggregated) and not q.group_by:
+                raise NotImplementedError("a correlated IN / EXISTS subquery with an aggregate needs a GROUP BY: "
+                                          "without one it is a single row even for an empty correlation group")
+            if (q.group_by or aggregated) and any(op != "=" for _, op, _ in corr):
+                raise NotImplementedError("a correlated subquery with GROUP BY or an aggregate is correlated by "
+                                          "equality keys only")
+            if q.group_by or aggregated:
+                extra_groups = [inner for inner, _, _ in corr]
+            if q.distinct or q.order_by or q.limit is not None or q.offset is not None or \
+                    any(e.contains_window() for e, _ in items):
+                raise NotImplementedError("LIMIT, ORDER BY, DISTINCT and window functions are not supported in a "
+                                          "correlated subquery")
+            self._corr[-1][:0] = [(inner, op, outer, len(items) + k) for k, (inner, op, outer) in enumerate(corr)]
+            items = items + [(inner, f"__corr{k}") for k, (inner, _, _) in enumerate(corr)]
         aliases = {a: e for e, a in items if a}
         # window calls of ORDER BY, bound where the SELECT list's are (they may read aggregates too)
         order_windows = {j: self.bind_expr(e, plan.schema) for j, (e, _, _) in enumerate(q.order_by or [])
@@ -116,6 +210,9 @@ class Binder:
         having = self.bind_expr(q.having, plan.schema, aliases) if q.having is not None else None
         if having is not None and having.contains_window():
             self.err("Window functions are not allowed in HAVING")
+        if self._joins[-1]:
+            raise NotImplementedError("a correlated scalar subquery in HAVING is not supported; use it in WHERE or "
+                                      "the SELECT list")
         is_agg = bool(q.group_by) or any(e.contains_agg() for e, _ in items) or \
             (having is not None and having.contains_agg()) or any(w.contains_agg() for w in order_windows.values())
 
@@ -131,8 +228,11 @@ class Binder:
                     group_exprs.append(aliases[g.parts[0]])
                 else:
                     group_exprs.append(self.bind_expr(g, plan.schema))
+            group_exprs += [x for x in extra_groups if all(x.display() != g.display() for g in group_exprs)]
             if any(g.contains_window() for g in group_exprs):
                 self.err("Window functions are not allowed in GROUP BY")
+            if any(g.contains_subquery() for g in group_exprs):
+                raise NotImplementedError("a subquery in GROUP BY is not supported")
             agg_calls: List[PyExpr] = []
 
             def collect(e: PyExpr):
@@ -231,6 +331,8 @@ class Binder:
                     b = P.col(f.qualifier, f.getName(), f.sql_type)
                 else:
                     b = self.bind_expr(e, plan.schema, order_by_fallback=items)
+                if b.contains_subquery():
+                    raise NotImplementedError("a subquery in ORDER BY is not supported")
                 keys.append((b, asc, (not asc) if nulls_first is None else nulls_first))
             plan = P.Sort(plan, keys)
         if q.limit is not None or q.offset is not None:
@@ -287,6 +389,8 @@ class Binder:
                     pairs.append((P.col(lf[0].qualifier, c, lf[0].sql_type), P.col(rf[0].qualifier, c, rf[0].sql_type)))
                 return P.Join(left, right, src.how, pairs, None)
             cond = self.bind_expr(src.on, scope)
+            if cond.contains_subquery():
+                raise NotImplementedError("a subquery in a JOIN's ON clause is not supported")
             pairs, residual = [], []
             holder = P.LogicalPlan()
             holder.schema = scope
@@ -338,12 +442,18 @@ class Binder:
                     for ex, al in order_by_fallback:
                         if al == name:
                             return P.col(None, name, ex.sql_type)
+                outer = self._outer_column(e.parts)
+                if outer is not None:
+                    return outer
                 self.err(f"Schema error: No field named {name}. Valid fields are "
                          f"{', '.join(f.getQualifiedName() for f in scope)}.")
             qual, name = parts[-2], parts[-1]
             hits = [f for f in scope if f.getName() == name and f.qualifier == qual]
             if len(hits) >= 1:
                 return P.col(qual, name, hits[0].sql_type)
+            outer = self._outer_column(e.parts)
+            if outer is not None:
+                return outer
             self.err(f"Schema error: No field named {qual}.{name}. Valid fields are "
                      f"{', '.join(f.getQualifiedName() for f in scope)}.")
         rec = lambda x: self.bind_expr(x, scope, aliases, order_by_fallback)  # noqa: E731
@@ -402,6 +512,8 @@ class Binder:
             return PyExpr("case", ty, args=args)
         if k == "window":
             return self._bind_window(e, rec)
+        if k in ("insubquery", "exists", "scalarsubquery"):
+            return self._bind_subquery(e, scope, rec)
         if k == "func":
             name = e.name
             if name in _WINDOW_ONLY:
@@ -452,6 +564,104 @@ class Binder:
                 return self._bind_math(name, args)
             self.err(f"Function {name} is outside the int64/float64 hot path of this layer")
         self.err(f"Unsupported expression {k}")
+
+    # -- subqueries -----------------------------------------------------------------------------
+    def _outer_column(self, parts) -> Optional[PyExpr]:
+        """a column of the immediately enclosing block, for the WHERE of a correlated subquery"""
+        def find(scope):
+            if len(parts) == 1:
+                hits = [f for f in scope if f.getName() == parts[0] or
+                        (not self.case_sensitive and f.getName().lower() == parts[0].lower())]
+            else:
+                hits = [f for f in scope if f.getName() == parts[-1] and f.qualifier == parts[-2]]
+            if len({(h.qualifier, h.getName()) for h in hits}) > 1:
+                self.err(f"Schema error: Ambiguous reference to unqualified field {parts[-1]}")
+            return hits[0] if hits else None
+
+        if self._outer and self._outer[-1] is not None:
+            f = find(self._outer[-1])
+            if f is not None:
+                return PyExpr("column", f.sql_type, qualifier=f.qualifier, name=f.getName(), value=_OUTER)
+        if any(scope is not None and find(scope) is not None for scope in self._outer[:-1]):
+            raise NotImplementedError(f"the column {'.'.join(parts)} belongs to a block that encloses this one "
+                                      "further out, or is used outside a subquery's WHERE: a correlated subquery "
+                                      "may refer to the immediately enclosing block, in its WHERE only")
+        return None
+
+    def _bind_subquery(self, e: Node, scope, rec) -> PyExpr:
+        """[NOT] IN (SELECT ...), EXISTS (SELECT ...) and (SELECT ...): the body is bound and optimised on its
+        own; correlated conjuncts of its WHERE become equality keys (inner = outer) and pair terms (the other
+        comparisons), and the IN's own x = y is the key of an uncorrelated IN, a pair term of a correlated one."""
+        from .optimizer import optimize
+        self._outer.append(scope)
+        self._corr.append([])
+        self._kind.append({"insubquery": "in", "exists": "exists", "scalarsubquery": "scalar"}[e.kind])
+        try:
+            body = self.bind_query(e.query, self._ctes[-1] if self._ctes else {})
+        finally:
+            self._outer.pop()
+            self._kind.pop()
+            corr = self._corr.pop()
+        count_kind = corr.pop() if e.kind == "scalarsubquery" and corr else None
+        body = optimize(body)
+        width = len(body.schema) - len(corr)
+        keys = [(outer, out) for _, op, outer, out in corr if op == "="]
+        terms = [(outer, out, _FLIP[op], True) for _, op, outer, out in corr if op != "="]
+        if e.kind == "scalarsubquery":
+            if width != 1:
+                self.err(f"A scalar subquery returns one column, not {width}")
+            ty = body.schema[0].sql_type
+            if corr:
+                return self._join_scalar(body, keys, count_kind, ty)
+            if ty in _TEMPORAL:
+                raise NotImplementedError(f"a scalar subquery of type {ty} is not supported")
+            self.volatile = True                # its value is read when the statement is planned
+            return PyExpr("subquery", ty, name="scalar subquery", value=P.Subquery(body, "scalar", [], [], False))
+        if corr and not keys:
+            raise NotImplementedError("a correlated IN / EXISTS subquery needs an equality key: a conjunct "
+                                      "inner_expr = outer_expr in its WHERE")
+        null_aware = False
+        if e.kind == "insubquery":
+            if width != 1:
+                self.err(f"IN (subquery) takes a subquery of one column, not {width}")
+            x = rec(e.e)
+            if corr:
+                terms.append((x, 0, "=", False))
+            else:
+                keys, null_aware = [(x, 0)], True
+        names = [f for f in body.schema]
+        if any(o.sql_type == "VARCHAR" or names[k].sql_type == "VARCHAR" for o, k, _, _ in terms):
+            raise NotImplementedError("a correlated subquery compares VARCHAR expressions by equality keys only")
+        if len(terms) > P.MARK_MAX_TERMS:
+            raise NotImplementedError(f"a correlated subquery compares at most {P.MARK_MAX_TERMS} pairs of "
+                                      f"expressions other than by equality keys, not {len(terms)}")
+        spec = P.Subquery(body, "in" if e.kind == "insubquery" else "exists", [k for _, k in keys],
+                          [(k, op, where) for _, k, op, where in terms], null_aware)
+        out = PyExpr("subquery", "BOOLEAN", name="in subquery" if e.kind == "insubquery" else "exists",
+                     args=[o for o, _ in keys] + [o for o, _, _, _ in terms], value=spec)
+        return PyExpr("not", "BOOLEAN", args=[out]) if e.negated else out
+
+    def _join_scalar(self, body, keys, count_kind, ty) -> PyExpr:
+        """A correlated scalar subquery, decorrelated as DataFusion's scalar-subquery-to-join rule does: the body
+        grouped by its inner key expressions, LEFT JOINed onto the enclosing block's rows on the outer keys; the
+        value is its aggregate column, NULL for a row without a group, and COUNT's 0 there (COALESCE)."""
+        if count_kind == "mixed":
+            raise NotImplementedError("a correlated scalar subquery that uses COUNT inside an expression is not "
+                                      "supported; use the COUNT alone")
+        pairs = []
+        self._nsq += 1
+        alias = f"{_SQ_ALIAS}{self._nsq}"
+        for outer, k in keys:
+            if outer.kind != "column":
+                raise NotImplementedError(f"a correlated scalar subquery is joined on columns of the enclosing block, "
+                                          f"not on {outer.display()}")
+            f = body.schema[k]
+            pairs.append((outer, P.col(alias, f.getName(), f.sql_type)))
+        self._joins[-1].append((alias, body, pairs))
+        v = P.col(alias, body.schema[0].getName(), ty)
+        if count_kind == "count":
+            v = PyExpr("case", ty, args=[PyExpr("isnull", "BOOLEAN", args=[v]), P.lit(0), v.clone()])
+        return v
 
     # -- window calls ---------------------------------------------------------------------------
     def _bind_window(self, node, rec) -> PyExpr:
@@ -659,6 +869,38 @@ class Binder:
         if a.sql_type not in _TEMPORAL and b.sql_type not in _TEMPORAL:
             self.err("TIMESTAMPDIFF takes DATE or TIMESTAMP arguments")
         return PyExpr("scalarfn", "BIGINT", name="timestampdiff", args=[P.lit(unit), a, b])
+
+
+_SQ_ALIAS = "__sq"      # qualifier of a decorrelated scalar subquery joined onto a block (hidden from *)
+_OUTER = "outer"        # PyExpr.value of a column of the enclosing block, in a correlated subquery's WHERE
+_FLIP = {"=": "=", "!=": "!=", "<": ">", "<=": ">=", ">": "<", ">=": "<="}
+
+
+def _count_kind(e: PyExpr) -> Optional[str]:
+    """"count": the item is COUNT / REGR_COUNT itself (0 over no rows); "mixed": a COUNT inside an expression"""
+    if e.kind == "agg" and e.name in ("COUNT", "REGR_COUNT"):
+        return "count"
+    found = []
+
+    def walk(x):
+        if x.kind == "agg" and x.name in ("COUNT", "REGR_COUNT"):
+            found.append(x)
+        for c in x.args:
+            walk(c)
+
+    walk(e)
+    return "mixed" if found else None
+
+
+def _outer_columns(e: PyExpr) -> List[PyExpr]:
+    return [c for c in e.columns() if c.value == _OUTER]
+
+
+def _strip_outer(e: PyExpr) -> PyExpr:
+    out = e.clone()
+    for c in out.columns():
+        c.value = None
+    return out
 
 
 _RAND_FUNCS = ("RAND", "RANDOM", "RAND_INTEGER")

@@ -54,6 +54,11 @@ def push_filters(plan: P.LogicalPlan, preds: List[PyExpr]) -> P.LogicalPlan:
     if isinstance(plan, P.Filter):
         return push_filters(plan.inputs[0], preds + P.conjuncts(plan.predicate))
 
+    held = [p for p in preds if p.contains_subquery()]
+    if held:
+        # a subquery predicate stays at the block whose rows it marks (executor: MarkSource)
+        return _wrap(push_filters(plan, [p for p in preds if not p.contains_subquery()]), held)
+
     if isinstance(plan, P.TableScan):
         plan.filters.extend(preds)
         return plan

@@ -155,6 +155,18 @@ class PyExpr:
     def contains_window(self):
         return self.kind == "window" or any(c.contains_window() for c in self.children())
 
+    def contains_subquery(self):
+        return self.kind == "subquery" or any(c.contains_subquery() for c in self.children())
+
+    def subqueries(self, out=None) -> List["PyExpr"]:
+        """the subquery calls of this expression, outermost first (not those inside their bodies)"""
+        out = [] if out is None else out
+        if self.kind == "subquery":
+            out.append(self)
+        for c in self.children():
+            c.subqueries(out)
+        return out
+
     # -- display (DataFusion-style names: they become output column names)
     def display(self) -> str:
         k = self.kind
@@ -218,6 +230,8 @@ class PyExpr:
             return f"{self.name.lower()}({', '.join(a.display() for a in self.args)})"
         if k == "window":
             return f"{self.name}({'*' if self.name == 'COUNT' and not self.args else ', '.join(a.display() for a in self.args)}) {self.window_text()}"
+        if k == "subquery":
+            return self.value.display(self.args)
         return k
 
     __repr__ = display
@@ -263,9 +277,13 @@ class PyExpr:
             return RexType.Literal
         if self.kind == "alias":
             return RexType.Alias
+        if self.kind == "subquery" and self.value.kind == "scalar":
+            return RexType.ScalarSubquery
         return RexType.Call
 
     def getExprType(self):
+        if self.kind == "subquery":
+            return {"scalar": "ScalarSubquery", "in": "InSubquery", "exists": "Exists"}[self.value.kind]
         return {"column": "Column", "literal": "Literal", "alias": "Alias", "agg": "AggregateFunction",
                 "binary": "BinaryExpr", "not": "Not", "isnull": "IsNull", "isnotnull": "IsNotNull",
                 "negative": "Negative", "between": "Between", "inlist": "InList", "cast": "Cast",
@@ -360,6 +378,45 @@ class PyExpr:
         return self.value
 
 
+MARK_MAX_TERMS = 4        # pair terms of one b2_join_mark (include/b200sql.h)
+
+
+class Subquery:
+    """The body of a subquery call (PyExpr kind "subquery"; its args are the enclosing block's side).
+    kind: "in" | "exists" | "scalar".  The body's output columns are its select list, then the inner side of
+    each correlated conjunct.  keys: body column of each equality key (arg k is its outer side); terms:
+    (body column, cmp, where) of each pair term, whose outer side is arg len(keys) + t; the mark compares
+    outer <cmp> inner, and `where` marks a conjunct of the body's WHERE (a NULL rejects the candidate).
+    null_aware: an uncorrelated IN, whose key is the IN operand."""
+
+    def __init__(self, plan, kind, keys, terms, null_aware):
+        self.plan, self.kind, self.keys, self.terms, self.null_aware = plan, kind, list(keys), list(terms), null_aware
+
+    def display(self, args) -> str:
+        if self.kind == "scalar":
+            return "(<subquery>)"
+        if self.kind == "in" and self.null_aware:
+            return f"{args[0].display()} IN (<subquery>)"
+        return f"{'IN' if self.kind == 'in' else 'EXISTS'} (<subquery> ON {self.key_text(args)})"
+
+    def key_text(self, args) -> str:
+        names = [f.getName() for f in self.plan.schema]
+        parts = [f"{a.display()} = {names[k]}" for a, k in zip(args, self.keys)]
+        parts += [f"{a.display()} {op} {names[k]}" for a, (k, op, _) in zip(args[len(self.keys):], self.terms)]
+        return " AND ".join(parts)
+
+    def explain(self, args, indent) -> str:
+        pad = "  " * indent
+        head = f"{pad}Subquery: {self.kind.upper()}"
+        if self.keys:
+            names = [f.getName() for f in self.plan.schema]
+            head += f" keys=[{', '.join(f'{a.display()} = {names[k]}' for a, k in zip(args, self.keys))}]"
+            if self.terms:
+                head += " pair terms=[" + ", ".join(f"{a.display()} {op} {names[k]}" for a, (k, op, _) in
+                                                    zip(args[len(self.keys):], self.terms)) + "]"
+        return head + "\n" + self.plan.explain(indent + 1)
+
+
 def col(qualifier, name, sql_type):
     return PyExpr("column", sql_type, qualifier=qualifier, name=name)
 
@@ -450,6 +507,9 @@ class LogicalPlan:
 
     def explain(self, indent=0) -> str:
         lines = ["  " * indent + self.describe()]
+        for e in self.expressions():
+            for sq in e.subqueries():
+                lines.append(sq.value.explain(sq.args, indent + 1))
         for i in self.inputs:
             lines.append(i.explain(indent + 1))
         return "\n".join(lines)

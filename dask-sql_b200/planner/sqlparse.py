@@ -12,6 +12,7 @@ that crate cannot be built here (no rustc/cargo), so this is a small recursive-d
 
 Expressions: literals (incl. DATE '...', TIMESTAMP '...', INTERVAL '...' [unit]), [qualifier.]column,
 + - * / %, comparisons, AND OR NOT, IS [NOT] NULL, [NOT] BETWEEN, [NOT] IN (list), CAST(e AS type),
+e [NOT] IN (select), [NOT] EXISTS (select), (select) as a scalar value,
 e [NOT] LIKE | ILIKE 'pattern' [ESCAPE 'c'],
 CASE WHEN, EXTRACT(field FROM e), FLOOR / CEIL(e TO unit), function calls incl. aggregates with
 DISTINCT and FILTER (WHERE ...), and window calls  f(...) OVER ([PARTITION BY e, ...] [ORDER BY ...] [frame])
@@ -502,6 +503,9 @@ class Parser:
         while True:
             if self.at_op("=", "<>", "!=", "<", "<=", ">", ">="):
                 op = self.eat_op("=", "<>", "!=", "<", "<=", ">", ">=")
+                if (self.at_kw("ALL") or self.at_word("ANY", "SOME")) and self.toks[self.i + 1].val == "(":
+                    raise NotImplementedError("ANY / ALL / SOME (subquery) comparisons are not supported; write "
+                                              "[NOT] IN (SELECT ...) or [NOT] EXISTS (SELECT ...)")
                 e = Node("bin", op="!=" if op == "<>" else op, l=e, r=self.parse_add())
             elif self.at_kw("IS"):
                 self.i += 1
@@ -537,7 +541,9 @@ class Parser:
         self.expect_kw("IN")
         self.expect_op("(")
         if self.at_kw("SELECT", "WITH"):
-            self.error("IN (subquery) is outside the hot-path grammar")
+            q = self.parse_query()
+            self.expect_op(")")
+            return Node("insubquery", e=e, query=q, negated=negated)
         items = [self.parse_expr()]
         while self.eat_op(","):
             items.append(self.parse_expr())
@@ -602,9 +608,22 @@ class Parser:
         if self.eat_kw("NULL"):
             return Node("lit", value=None)
         if self.eat_op("("):
+            if self.at_kw("SELECT", "WITH"):                # (SELECT one_value ...) as an expression
+                q = self.parse_query()
+                self.expect_op(")")
+                return Node("scalarsubquery", query=q)
             e = self.parse_expr()
+            if self.at_op(","):
+                raise NotImplementedError("row values such as (a, b) IN (SELECT ...) are not supported; compare "
+                                          "one expression, or write a correlated EXISTS")
             self.expect_op(")")
             return e
+        if self.at_word("EXISTS") and self.toks[self.i + 1].val == "(" and self.toks[self.i + 2].kind == "kw" \
+                and self.toks[self.i + 2].val in ("SELECT", "WITH"):
+            self.i += 2
+            q = self.parse_query()
+            self.expect_op(")")
+            return Node("exists", query=q)
         if self.eat_kw("CAST"):
             self.expect_op("(")
             e = self.parse_expr()

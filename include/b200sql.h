@@ -525,6 +525,38 @@ int32_t b2_join_onepass(const b2_scan_t* scan, const int32_t* probe_keys, const 
                         const b2_col_t* build_cols, const int64_t* build_base, void* const* build_out,
                         uint32_t* const* build_valid, void* stream);
 
+/* ---- subquery mark: [NOT] IN (SELECT ...) / [NOT] EXISTS (SELECT ...) ------------------------ */
+/* The reference evaluates `x IN (SELECT y ...)` with series.isin (physical/rex/core/call.py:996-1030,
+ * InSubqueryOperation) and runs the LEFTSEMI / LEFTANTI joins DataFusion makes of EXISTS
+ * (physical/rel/logical/join.py:46-47, 146-229).  Here both are one mark per probe row, a three-valued
+ * BOOLEAN: out[i] = 1 (TRUE) or 0, validity bit clear for NULL.
+ *   candidates(i) = build rows of the table whose keys equal row i's (a NULL key equals nothing);
+ *   mark(i)       = OR over the candidates j of the AND of the pair terms
+ *                   scan.cols[terms[t].probe_col][i] <terms[t].cmp> terms[t].build[j]   (NULL if a side is;
+ *                   a term with B2_MARK_WHERE or-ed into cmp comes from the subquery's WHERE, and its NULL
+ *                   rejects the candidate as WHERE does, so only the IN's own x = y term is ever NULL; that
+ *                   term also takes a float NaN for NULL, as keys do, where WHERE terms compare NaN as IEEE);
+ *   B2_MARK_NULL_AWARE: the one probe key is the IN operand: with B2_MARK_BUILD_NONEMPTY a NULL key gives
+ *     NULL, and with B2_MARK_BUILD_HAS_NULL (the build side holds a NULL key) a FALSE mark becomes NULL.
+ * Rows that fail the scan's terms get FALSE.  Without pair terms every table kind is accepted (duplicate
+ * build keys are harmless); with pair terms the table must list every candidate: chained (dense 0), or
+ * direct-address (dense 1, unique keys).  Pair-term sides are B2_I64 or B2_F64, the same on both sides.
+ * out: uint8[scan.n]; out_valid: (scan.n+31)/32 words, every one written.  Arguments outside these rules
+ * return B2_ERR_ARG. */
+#define B2_MARK_MAX_TERMS       4
+#define B2_MARK_NULL_AWARE      1
+#define B2_MARK_BUILD_NONEMPTY  2
+#define B2_MARK_BUILD_HAS_NULL  4
+#define B2_MARK_WHERE           8   /* or-ed into b2_mark_term_t.cmp */
+typedef struct b2_mark_term {
+  int32_t  probe_col;   /* column of scan.cols */
+  b2_col_t build;       /* build-side values, indexed by build row */
+  int32_t  cmp;         /* B2_EQ .. B2_GE, | B2_MARK_WHERE */
+} b2_mark_term_t;
+int32_t b2_join_mark(const b2_scan_t* scan, const int32_t* probe_keys, const b2_jointable_t* jt,
+                     const b2_mark_term_t* terms, int32_t nterms, int32_t flags, uint8_t* out, uint32_t* out_valid,
+                     void* stream);
+
 /* ---- inner join fused with GLOBAL aggregates over both sides (C3, non-materialising) ---------- */
 /* One pass over the probe partition: predicate -> presence + payload lookup at the key offset ->
  * combine -> aggregate; no join row is materialised.  Replaces, fused, join.py:189-248 (merge:
